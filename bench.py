@@ -4,12 +4,14 @@ ray-samples/sec).  One "step" = one Trainer.step(): K1 sampling -> K4 fused PE+M
 input-gradient / losses / double back-prop -> K5 -> [C1 all-reduce] -> K6 AdamW+re-pack.
 
   python bench.py --gpus N --steps K --warmup W [--impl reference] [--precision bf16x3|bf16|fp32]
-                  [--workload default|scannet|c4|c5]
+                  [--workload default|scannet|c4|c5|grid] [--dump-outputs DIR]
 
 Prints ONE JSON line (contract in the task statement): metric/value/unit (device-resident inputs),
 e2e (public API with host frames, H2D + D2H inside the timed region), roofline (dominant kernel,
 CUDA-event timed inside the library), cpu_baseline (oracle port on the host cores), clocks.
-`--impl reference` times the CPU port of the reference's own step instead (rank 0 only)."""
+`--impl reference` times the CPU port of the reference's own step instead (rank 0 only).
+`--dump-outputs DIR` writes what the last timed step computed as DIR/<name>.npy (see dump_outputs), so that two builds
+run with the same arguments (same seeds, same inputs) can be compared output for output."""
 import argparse
 import json
 import os
@@ -34,7 +36,7 @@ WORKLOADS = {
     # configs[3]: synthetic 640x480, 4096 rays/frame x 64 samples
     "c4": dict(H=480, W=640, fx=577.87, fy=577.87, cx=319.5, cy=239.5, n_rays=4096, n_strat=56, n_surf=8,
                hidden=256, block=2, keyframes=8, name="synthetic 640x480 5x4096 rays x 64 samples"),
-    # configs[4]: wide MLP 512x8 (hidden 512, hidden_layers_block 4), 8192 rays/frame x 128 samples.  The tcgen05 kernels
+    # configs[4]: wide MLP 512x8 (hidden 512, hidden_layers_block 4), 8192 rays/frame x 128 samples.  The wgmma kernels
     # take hidden = 256 only: this model runs on the library's fp32 CUDA-core kernels (Trainer falls back with a warning)
     "c5": dict(H=480, W=640, fx=577.87, fy=577.87, cx=319.5, cy=239.5, n_rays=8192, n_strat=120, n_surf=8,
                hidden=512, block=4, keyframes=8, name="wide MLP 512x(4+4), synthetic 640x480 5x8192 rays x 128 samples"),
@@ -43,7 +45,9 @@ WORKLOADS = {
                  hidden=256, block=2, keyframes=1, grid_dim=200,
                  name="get_sdf_grid 200^3 lattice (8.0 M points, forward-only K2, lattice generated in-kernel), 256x(2+2) MLP"),
 }
-PEAKS_FALLBACK = dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0)
+# NVIDIA H100 SXM data sheet (700 W part): HBM3 bandwidth and dense BF16 tensor rate -- peaks, never reached figures
+PEAKS_FALLBACK = dict(hbm_gbs=3350.0, bf16_tflops=989.0)
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def load_peaks():
@@ -53,7 +57,7 @@ def load_peaks():
         d["_source"] = "measured (MEASURED_PEAKS.json)"
         return d
     d = dict(PEAKS_FALLBACK)
-    d["_source"] = "fallback (B200_PROFILING.md)"
+    d["_source"] = "fallback (H100 SXM data sheet)"
     return d
 
 
@@ -78,8 +82,8 @@ def make_config(wl, precision, rng_mode):
                  "orien_loss": 0},
         "pose_refine": {"pose_lr": 0.0004},
         "b200": {"precision": precision, "rng_mode": rng_mode,
-                 # chunk = a whole number of 148-SM waves of 128-point tiles (no partial last wave)
-                 "max_points": (148 * 128 * 8 if wl.get("grid_dim") else 148 * 128 * 4 if wl["n_rays"] > 1000 else 32768)},
+                 # chunk = a whole number of 132-SM (H100 SXM) waves of 128-point tiles (no partial last wave)
+                 "max_points": (132 * 128 * 8 if wl.get("grid_dim") else 132 * 128 * 4 if wl["n_rays"] > 1000 else 32768)},
     }
 
 
@@ -122,6 +126,26 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy: float64 stays float64, everything else becomes float32.  When the
+    arrays would take more than DUMP_LIMIT_BYTES, every array above an equal share of the limit is replaced by a fixed
+    sample of its flattened elements (seeded generator: the same indices for the same length, in increasing order)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    host = {}
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if torch.is_tensor(a) else np.asarray(a)
+        host[name] = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+    total = sum(a.nbytes for a in host.values())
+    share = DUMP_LIMIT_BYTES // max(len(host), 1)
+    for name, a in host.items():
+        if total > DUMP_LIMIT_BYTES and a.nbytes > share:
+            k = share // a.itemsize
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=k, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def flops_per_point(E, Hd, B, units_only_chain=False):
     """SURVEY.md 8d: training step = 2*(6 F_MAC - 2 E Hd) with F_MAC = E Hd + 2B Hd^2 + (Hd+E) Hd + Hd."""
     f_mac = E * Hd + 2 * B * Hd * Hd + (Hd + E) * Hd + Hd
@@ -131,7 +155,7 @@ def flops_per_point(E, Hd, B, units_only_chain=False):
 def host_threads():
     """One compute thread per PHYSICAL core this process may use (torch's own default; torchrun exports
     OMP_NUM_THREADS=1, which the CPU arm overrides).  Hyper-thread siblings are left idle: with 2 x 64 logical CPUs the
-    reference step ran 2x slower and 3x noisier on 128 threads than on 64 (profiles/r02_summary.md)."""
+    reference step ran 2x slower and 3x noisier on 128 threads than on 64."""
     try:
         n = len(os.sched_getaffinity(0))
     except AttributeError:
@@ -184,7 +208,7 @@ def time_cpu(stepper, warmup, steps):
 
 def run_reference_arm(args, wl, rank):
     """`--impl reference`: the reference's own CPU implementation of the step on this box's host cores (tier rule),
-    same workload config, metric and unit as the B200 arm.  Rank 0 only; the other ranks exit without work."""
+    same workload config, metric and unit as the CUDA arm.  Rank 0 only; the other ranks exit without work."""
     if rank != 0:
         return
     cores = host_threads()
@@ -211,8 +235,8 @@ def run_reference_arm(args, wl, rank):
 
 
 def load_traffic(precision, workload):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture of the same launch shape
-    (profiles/chain_traffic.json, written by tools/update_traffic.py from an .ncu-rep; carries its provenance)."""
+    """DRAM bytes per launch of the dominant kernel from a committed profiler record of the same launch shape
+    (profiles/chain_traffic.json, with its provenance); None when there is no record."""
     f = os.path.join(ROOT, "profiles", "chain_traffic.json")
     try:
         rec = json.load(open(f)).get(precision, {}).get(workload)
@@ -253,10 +277,12 @@ def run_grid_bench(args, wl, dev, rank, world, dist):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        tr.get_sdf_grid()
+        grid = tr.get_sdf_grid()
     e1.record()
     torch.cuda.synchronize(dev)
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"sdf_grid": grid})
     clocks = sampler.stop() if rank == 0 else None
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if dist is not None:
@@ -284,7 +310,7 @@ def run_grid_bench(args, wl, dev, rank, world, dist):
         eng.profile(False)
         n_l = max(pr["n_chain"], 1)
         pts_per_launch = 3.0 * n_pts / n_l
-        fwd_flops_pt = 2.0 * 256 * 256 * (2 * wl["block"] + 3)          # 7 UMMA products per point (E padded to 256)
+        fwd_flops_pt = 2.0 * 256 * 256 * (2 * wl["block"] + 3)          # 7 MMA products per point (E padded to 256)
         chain_ms = pr["chain_ms"] / n_l
         ach = fwd_flops_pt * pts_per_launch / (chain_ms * 1e-3) / 1e12
         peak = peaks.get("bf16_tflops", PEAKS_FALLBACK["bf16_tflops"])
@@ -320,7 +346,11 @@ def main():
                     choices=["bf16x3g", "bf16x3", "bf16", "fp32"])
     ap.add_argument("--workload", default="default", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32 / float64, <= 64 MB)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.steps < 1):
+        ap.error("--dump-outputs needs at least one timed step of the CUDA implementation (--steps >= 1, no --impl reference)")
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", 0))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
@@ -405,9 +435,15 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        tr.step(sync=False)
+        losses, _ = tr.step(sync=False)
     e1.record()
     torch.cuda.synchronize(dev)
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed step receives: its losses, the per-sample sdf and loss it computed, and the
+        # parameters its AdamW update left behind
+        out = {k: v for k, v in losses.items()}
+        out.update(sdf=tr.last_sdf, loss_mat=tr.last_loss_mat, params=tr.sdf_map.flat_parameters())
+        dump_outputs(args.dump_outputs, out)
     launches = launches_per_step * args.steps
     ms = e0.elapsed_time(e1)
     barrier()
@@ -476,7 +512,7 @@ def main():
     # ---------------- roofline of the dominant kernel (rank 0, events inside the library) -------------
     roof = None
     peaks = load_peaks()
-    prec = eng.precision                     # the model's actual precision (fp32 when the tcgen05 path refused the shape)
+    prec = eng.precision                     # the model's actual precision (fp32 when the tensor-core path refused the shape)
     if prec != "fp32":
         tr.use_graph = False                 # the event hooks live in the library's host code
         eng.profile(True)
@@ -486,7 +522,7 @@ def main():
         eng.profile(False)
         tr.use_graph = True
         lay_E = 3 + 2 * 21 * 6
-        n_units = 4 * (2 * wl["block"] + 2) + 2                     # UMMA products of the chain kernel
+        n_units = 4 * (2 * wl["block"] + 2) + 2                     # MMA products of the chain kernel
         n_prof_steps = 20
         pts_per_launch = pts_per_step * n_prof_steps / max(pr["n_chain"], 1)    # a step is cut into max_points chunks
         tiles = int((pts_per_launch + 127) // 128)
@@ -495,8 +531,8 @@ def main():
         dw_ms = pr["dw_ms"] / max(pr["n_dw"], 1)
         ach = chain_flops / (chain_ms * 1e-3) / 1e12
         peak = peaks.get("bf16_tflops", PEAKS_FALLBACK["bf16_tflops"])
-        roof = {"kernel": {"bf16x3": "tc_chain_kernel<3,1,false>", "bf16x3g": "tc_chain_kernel<3,1,true>",
-                           "bf16": "tc_chain_kernel<1,1,false>"}[prec], "bound": "tensor",
+        roof = {"kernel": {"bf16x3": "tc_chain_kernel<3,false,1>", "bf16x3g": "tc_chain_kernel<3,true,1>",
+                           "bf16": "tc_chain_kernel<1,false,1>"}[prec], "bound": "tensor",
                 "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
                 "peak_source": peaks["_source"] + " burst bf16", "ms_per_launch": chain_ms,
                 "algorithmic_flops_per_launch": chain_flops, "tiles": tiles,
@@ -509,7 +545,7 @@ def main():
             roof["hbm_frac"] = roof["hbm_achieved_gbs"] / hbm_peak
 
     else:
-        # fp32 CUDA-core path (models the tcgen05 kernels do not take, e.g. hidden 512): whole-step figure against the
+        # fp32 CUDA-core path (models the wgmma kernels do not take, e.g. hidden 512): whole-step figure against the
         # same tensor peak the north-star names -- the register-tiled SGEMM cannot approach it; reported, not hidden
         lay_E = 3 + 2 * 21 * 6
         fpp = flops_per_point(lay_E, wl["hidden"], wl["block"])
@@ -518,8 +554,8 @@ def main():
         roof = {"kernel": "sgemm_kernel + element-wise kernels (fp32 CUDA-core path, simt_path.cu), whole step",
                 "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
                 "peak_source": peaks["_source"] + " burst bf16", "step_flops_per_point": fpp,
-                "note": "fp32 FFMA peak of the part is ~74 TFLOP/s (148 SMs x 128 lanes x 2 x 1.965 GHz): %.0f %% of that"
-                        % (100.0 * ach / 74.4)}
+                "note": "fp32 FFMA peak of the H100 SXM is ~67 TFLOP/s (132 SMs x 128 lanes x 2 x 1.98 GHz): %.0f %% of that"
+                        % (100.0 * ach / 66.9)}
 
     # ---------------- data-parallel parity (N > 1): replicas identical, fused exchange == NCCL all-reduce -----------
     xchg = None
@@ -588,7 +624,7 @@ def main():
                               "none" if world == 1 else
                               "fused into the weight-gradient kernel over NVLink multicast (multimem.red) + 1 barrier" if used_multicast
                               else "one NCCL all-reduce of the packed gradient%s" % (" inside the step graph" if tr._nccl_in_graph else ""))),
-                          "l2": "no explicit flush: keyframe buffer %.0f MB and per-step side state %.0f MB both exceed the 126 MB L2"
+                          "l2": "no explicit flush: keyframe buffer %.0f MB, per-step side state %.0f MB (H100 L2: 50 MB)"
                                 % (wl["keyframes"] * wl["H"] * wl["W"] * 16 / 1e6, pts_per_step * 0.041)},
                "clocks": clocks,
                "e2e": {"value": e2e_val, "unit": "ray-samples/s", "ms_per_step": e2e_ms / args.steps,

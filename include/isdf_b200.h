@@ -1,5 +1,5 @@
 /*
- * isdf_b200 -- C ABI of the B200 (sm_100a) implementation of the iSDF training hot path.
+ * isdf_b200 -- C ABI of the H100 (sm_90a) implementation of the iSDF training hot path.
  *
  * The reference (facebookresearch/iSDF) is pure Python/PyTorch and has no FFI of its own
  * (SURVEY.md 8b); every entry point below replaces a block of reference Python that the
@@ -31,14 +31,14 @@ typedef enum {
   ISDFB_OK = 0,
   ISDFB_ERR_ARG = -1,        /* bad argument / unsupported configuration */
   ISDFB_ERR_CUDA = -2,       /* CUDA runtime error (message carries cudaGetErrorString) */
-  ISDFB_ERR_CAPACITY = -3,   /* batch larger than the workspace / TMEM / smem budget */
+  ISDFB_ERR_CAPACITY = -3,   /* batch larger than the workspace / shared-memory budget */
   ISDFB_ERR_STATE = -4       /* call order violated (e.g. weights not packed) */
 } isdfb_status;
 
 typedef enum {
   ISDFB_PREC_FP32 = 0,       /* fp32 CUDA-core path (exact-parity mode, also the on-device check) */
-  ISDFB_PREC_BF16X3 = 1,     /* tcgen05 kind::f16, bf16 hi/lo split, 3 MMAs per product (~fp32) */
-  ISDFB_PREC_BF16 = 2,       /* tcgen05 kind::f16, single bf16 pass (fast mode) */
+  ISDFB_PREC_BF16X3 = 1,     /* wgmma bf16 -> f32, bf16 hi/lo split, 3 MMAs per product (~fp32) */
+  ISDFB_PREC_BF16 = 2,       /* wgmma bf16 -> f32, single bf16 pass (fast mode) */
   ISDFB_PREC_BF16X3G = 3     /* as BF16X3 for every product of the sweeps S1..S4 (sdf, d sdf/dx, losses identical), but
                                 the operands handed to the weight-gradient products, the S3 read-back of delta_l and
                                 zbar2_l are single bf16: half the per-point side state in HBM; weight gradients carry
@@ -276,7 +276,7 @@ int isdfb_profile_read(isdfb_ctx* ctx, double* chain_ms, double* dw_ms, int64_t*
  * d sdf/dx, 2 training.  steps_out receives 8 int32 per step: weight unit, orientation (0: X W^T, 1: X W), epilogue kind
  * (0 RAW, 1 S1, 2 S1_LAST, 3 S2, 4 S2_END, 5 S3, 6 S3_LAST, 7 S4), hidden layer, partial-sum array written, partial-sum
  * array added (-1 none), flags (1 accumulate, 2 then-write-e, 4 then-write-abar_e, 8 first / 16 last embedding half),
- * (generated half << 8 | output half).  Returns the step count; < 0: bad argument (-1), shape not taken by the tcgen05
+ * (generated half << 8 | output half).  Returns the step count; < 0: bad argument (-1), shape not taken by the tensor-core
  * path (-2), buffer too small (-4).  The sweeps are SURVEY.md 8a's S1..S4 (fc_map.py:94-111, 12-22; trainer.py:981). */
 int isdfb_debug_program(int32_t n_freqs, int32_t hidden, int32_t block, int32_t mode, int32_t* steps_out,
                         int32_t max_steps);

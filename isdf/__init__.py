@@ -1,7 +1,7 @@
 """Drop-in alias: `from isdf.modules import trainer` (reference train.py:16) resolves to isdf_b200.
 
 Put this repo's root on sys.path BEFORE the reference checkout and the reference drivers
-(isdf/train/train.py, train_vis.py, batch_train) import the B200 implementation unchanged:
+(isdf/train/train.py, train_vis.py, batch_train) import this implementation unchanged:
 
 * `isdf.modules`, `isdf.geometry`, `isdf.datasets`, `isdf.eval` are this repo's packages;
 * every other sub-package the drivers import (`isdf.visualisation`, `isdf.train`, `isdf.ros_utils`, ...) and
@@ -53,7 +53,7 @@ def _fallback_getattr(mod, ref_file):
             # never silent: a name of a mirrored (hot-path) module that is served by the reference's Python code is worth
             # knowing about -- it is either out-of-scope tooling (to_trimesh, plotting helpers) or a gap in this package
             state["warned"].add(name)
-            warnings.warn("isdf_b200: %s.%s is not provided by the B200 implementation; using the reference's %s"
+            warnings.warn("isdf_b200: %s.%s is not provided by this implementation; using the reference's %s"
                           % (mod.__name__, name, ref_file), stacklevel=2)
         return val
     return __getattr__

@@ -1,4 +1,4 @@
-"""isdf_b200 -- B200 (sm_100a) implementation of the iSDF continual-training hot path.
+"""isdf_b200 -- H100 (sm_90a) implementation of the iSDF continual-training hot path.
 
 Host side mirrors the reference's Python interface (isdf.modules.trainer.Trainer and
 isdf.modules.{fc_map,embedding,sample,loss,render}); compute goes through the C ABI in

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI declared in include/isdf_b200.h.
 
-The shared library is built in-tree by `__graft_entry__.build()` (nvcc, sm_100a) as
+The shared library is built in-tree by `__graft_entry__.build()` (nvcc, sm_90a) as
 isdf_b200/lib/libisdf_b200.so.  There is NO fallback: if the library is missing or a
 symbol is absent, importing/using the product path raises.
 """
@@ -88,7 +88,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             "isdf_b200: CUDA library %s not found. Build it with `python -c 'import __graft_entry__ as g; "
-            "g.build()'` (nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+            "g.build()'` (nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)      # AttributeError if the symbol is not exported

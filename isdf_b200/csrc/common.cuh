@@ -1,4 +1,4 @@
-// Shared declarations for the isdf_b200 kernels (sm_100a only).
+// Shared declarations for the isdf_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -8,7 +8,7 @@
 #include "../../include/isdf_b200.h"
 
 #define ISDFB_MAX_HIDDEN_LAYERS 10   // 2*block + 2, block <= 4
-#define ISDFB_TILE 128               // points per tile (UMMA M)
+#define ISDFB_TILE 128               // points per tile (two wgmma M = 64 slabs)
 #define ISDFB_NDIRS 21
 
 // One hidden layer of the packed (internal) parameter layout.  All matrices are fp32,

@@ -2,7 +2,7 @@
 //
 // This is the exact-parity mode (ISDFB_PREC_FP32): every product is an fp32 FFMA, the same
 // arithmetic the reference's PyTorch path performs (TF32 is off by default in torch), so it
-// tracks the reference to ~1e-6.  It also serves as the on-device check for the tcgen05 path.
+// tracks the reference to ~1e-6.  It also serves as the on-device check for the tensor-core path.
 // Activations live in HBM as row-major [points][width] fp32 arrays; one GEMM kernel template
 // covers  Y = X W^T (S1,S3),  Y = X W (S2,S4)  and  dW += X^T Y (weight gradients, split-K).
 #include "common.cuh"

@@ -1,4 +1,4 @@
-// Argument block and step program of the tcgen05 chain kernel (tc_chain.cu).
+// Argument block and step program of the wgmma chain kernel (tc_chain.cu).
 #pragma once
 #include "tc_common.cuh"
 
@@ -49,10 +49,9 @@ struct TcChainArgs {
   int32_t tile0;             // ... starting at this tile of the chunk
   int32_t prefetch;          // 1: bulk-prefetch the next step's side arrays into L2 (producer warp)
   int32_t stagger;           // 1: per-CTA rotation of the K order (rot_kstep) against L2 hot-spotting on the weights
-  int32_t wide;              // 1: epilogue variant with 16-column TMEM loads (two interleaved chains per chunk)
   int32_t ablate;            // DEV ONLY (env ISDFB_ABLATE + a build with -DISDFB_DEV_ABLATE; results invalid): 1 no dW-layout stores, 2 no aux stores,
-                             // 4 no sigma stores, 8 no side loads, 16 relu instead of softplus, 32 no A-image stores,
-                             // 64 no PE-Jacobian / abar_e math -- timing ablations for profiles/
+                             // 4 no sigma stores, 8 no sigma loads in S2, 16 relu instead of softplus, 32 no A-image stores,
+                             // 64 no PE-Jacobian / abar_e math, 256 no MMA, 512 no weight traffic -- timing ablations
   int64_t n_points;          // real points in this chunk
   int64_t p0;                // global index of the chunk's first point (sample index r*S+j)
   PEParams pe;

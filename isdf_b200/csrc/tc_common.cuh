@@ -1,11 +1,11 @@
-// sm_100a primitives for the tensor-core path: mbarrier, bulk (TMA) copies, TMEM management,
-// tcgen05.mma / tcgen05.ld wrappers, UMMA shared-memory and instruction descriptors, and the
-// operand-image layouts shared by the chain kernel, the weight-gradient kernel and the packer.
+// sm_90a primitives for the tensor-core path: mbarrier, bulk (TMA) copies, wgmma wrappers and
+// shared-memory matrix descriptors, and the operand-image layouts shared by the chain kernel, the
+// weight-gradient kernel and the packer.
 #pragma once
 #include "common.cuh"
 
 #define TC_H 256                 // hidden width == padded embedding width supported by this path
-#define TC_TILE 128              // points per tile (UMMA M)
+#define TC_TILE 128              // points per tile (two warpgroups x wgmma M = 64)
 #define TC_TILE_FLOATS (TC_H * TC_TILE)
 
 // ---- layouts --------------------------------------------------------------------------------
@@ -19,7 +19,7 @@ __host__ __device__ __forceinline__ uint32_t kmajor_off_bytes(uint32_t rows, uin
 __host__ __device__ __forceinline__ uint32_t aux_off_floats(uint32_t f, uint32_t p) {
   return (f >> 2) * 512u + p * 4u + (f & 3u);
 }
-// (3) per-tile bf16 "dW layout": [p/16][f/8][16 pts][8 f] -> each 16-point slice (one UMMA K step
+// (3) per-tile bf16 "dW layout": [p/16][f/8][16 pts][8 f] -> each 16-point slice (one wgmma K step
 //     of the weight-gradient GEMM) is 8 KB contiguous and is an MN-major operand with
 //     SBO (next 8 features) = 256 B, LBO (next 8 points) = 128 B.
 __host__ __device__ __forceinline__ uint32_t dwl_off_bytes(uint32_t f, uint32_t p) {
@@ -72,15 +72,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   return ok != 0;
 }
 // Spin on the phase; a wait that lasts > ~2 s of SM clocks is a protocol bug -> trap (surfaces as a CUDA
-// error on the host instead of hanging the GPU).
+// error on the host instead of hanging the GPU).  No printf here: it is a function call, and ptxas serialises
+// every wgmma of a kernel that contains one.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("isdf_b200: mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();
   }
 }
 // global -> shared bulk copy (TMA, 1-D), completion signalled on an mbarrier
@@ -95,66 +93,62 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma (warpgroup MMA, accumulators in registers) -------------------------------------------
+// Accumulator fragment of m64nNk16 (f32) for thread t of the warpgroup (warp w = t / 32, lane l):
+//   d[4 i + 2 rh + e]  ->  row 16 w + l / 4 + 8 rh,  column 8 i + 2 (l % 4) + e.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kN> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kN) : "memory"); }
+// pins the accumulator registers at this point of the program: reads of d after a wgmma_wait cannot be hoisted
+// above it (the asm of the MMA itself "produces" d as far as the compiler knows)
+template <int kRegs> __device__ __forceinline__ void wgmma_fence_operands(float* d) {
+#pragma unroll
+  for (int i = 0; i < kRegs; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// all previously issued tcgen05.mma of this thread done -> arrive(1) on the mbarrier
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate; kTA / kTB = 1: the operand is MN-major
+template <int kTA, int kTB>
+__device__ __forceinline__ void wgmma_m64n256k16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, %131, %132;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTA), "n"(kTB));
 }
-// 32 lanes x 32 columns of fp32 -> 32 registers per thread (thread = lane/row)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
+template <int kTA, int kTB>
+__device__ __forceinline__ void wgmma_m64n16k16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, p, 1, 1, %11, %12;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTA), "n"(kTB));
 }
 
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 8 columns
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 // sigma in [0,1] as unorm16 (abs error 7.6e-6; 0 and 1 exact): 8 values <-> 16 B.
 // Conversions stay on the FMA/ALU pipes (magic-number rounding), not on the quarter-rate XU pipe.
 __device__ __forceinline__ uint4 pack_unorm16x8(const float* s) {
@@ -179,6 +173,16 @@ __device__ __forceinline__ void unpack_unorm16x8(const uint4& v, float* s) {
     s[2 * i] = fmaf(__uint_as_float(__byte_perm(w[i], 0x4B000000u, 0x7610)), c, k);
     s[2 * i + 1] = fmaf(__uint_as_float(__byte_perm(w[i], 0x4B000000u, 0x7632)), c, k);
   }
+}
+// the same unorm16 code for two values <-> 4 B
+__device__ __forceinline__ uint32_t pack_unorm16x2(float s0, float s1) {
+  const uint32_t a = __float_as_uint(fmaf(s0, 65535.f, 8388608.f)), b = __float_as_uint(fmaf(s1, 65535.f, 8388608.f));
+  return __byte_perm(a, b, 0x5410);
+}
+__device__ __forceinline__ void unpack_unorm16x2(uint32_t w, float& s0, float& s1) {
+  const float c = 1.525902e-05f, k = -8388608.f * c;
+  s0 = fmaf(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7610)), c, k);
+  s1 = fmaf(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7632)), c, k);
 }
 // warp-specialised register re-allocation (whole warpgroups = 4 consecutive warps): the helper warpgroup gives
 // registers back, the epilogue warpgroups take them
@@ -210,25 +214,24 @@ __device__ __forceinline__ void grad_add(float* p, float v, int mc) {
   if (mc) asm volatile("multimem.red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
   else asm volatile("red.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
 }
+__device__ __forceinline__ void grad_add2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
 __device__ __forceinline__ void grad_add4(float* p, float a, float b, float c, float d, int mc) {
   if (mc) asm volatile("multimem.red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
   else asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
 // ---- descriptors --------------------------------------------------------------------------------
-// shared-memory matrix descriptor, SWIZZLE_NONE (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start>>4   [16,30) LBO>>4   [32,46) SBO>>4   [46,48) version=1   [61,64) layout=0
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// wgmma shared-memory matrix descriptor, no swizzle (8x8 core matrices of 128 contiguous bytes):
+//   [0,14) start>>4   [16,30) LBO>>4   [32,46) SBO>>4   [62,64) layout = 0
+// K-major: LBO = next 8 K, SBO = next 8 rows.  MN-major: LBO = next 8 K, SBO = next 8 M/N.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
-}
-// instruction descriptor for kind::f16: D=f32, A=B=bf16, M x N, optional MN-major operands
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // ---- bf16 split -----------------------------------------------------------------------------------
@@ -257,6 +260,15 @@ __device__ __forceinline__ void split8(const float* x, uint4& hi, uint4& lo) {
   }
   hi = make_uint4(h[0], h[1], h[2], h[3]);
   lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+// two fp32 -> packed bf16 hi and bf16 lo
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  hi = cvt_bf16x2(x0, x1);
+  lo = cvt_bf16x2(x0 - __uint_as_float(hi << 16), x1 - __uint_as_float(hi & 0xFFFF0000u));
+}
+__device__ __forceinline__ void unpack2(uint32_t w, float& x0, float& x1) {
+  x0 = __uint_as_float(w << 16);
+  x1 = __uint_as_float(w & 0xFFFF0000u);
 }
 __device__ __forceinline__ uint4 pack8_hi(const float* x) {
   return make_uint4(cvt_bf16x2(x[0], x[1]), cvt_bf16x2(x[2], x[3]), cvt_bf16x2(x[4], x[5]), cvt_bf16x2(x[6], x[7]));

@@ -82,7 +82,7 @@ extern "C" int isdfb_debug_program(int32_t n_freqs, int32_t hidden, int32_t bloc
   lay.H = hidden;
   lay.block = block;
   lay.L = 2 * block + 2;
-  if (lay.H != TC_H || lay.E > TC_MAX_EH * TC_H) return -2;          // shapes the tcgen05 path refuses
+  if (lay.H != TC_H || lay.E > TC_MAX_EH * TC_H) return -2;          // shapes the tensor-core path refuses
   TcChainArgs* a = new (std::nothrow) TcChainArgs();
   if (!a) return -3;
   memset(a, 0, sizeof(*a));
@@ -180,7 +180,6 @@ int tc_create(isdfb_ctx* ctx) {
     a.mode = mode; a.L = L; a.ic = ic; a.E = lay.E;
     a.prefetch = getenv("ISDFB_NO_PREFETCH") ? 0 : 1;
     a.stagger = getenv("ISDFB_STAGGER") ? atoi(getenv("ISDFB_STAGGER")) : 1;
-    a.wide = getenv("ISDFB_EPI_WIDE") ? atoi(getenv("ISDFB_EPI_WIDE")) : 1;
     a.ablate = getenv("ISDFB_ABLATE") ? atoi(getenv("ISDFB_ABLATE")) : 0;
     a.dbg_clock = tc->dbg_clock;
     a.pe = ctx->pe;
@@ -196,7 +195,6 @@ int tc_create(isdfb_ctx* ctx) {
     a.arr_part = 0; a.arr_e32 = n_part; a.arr_hlast = n_part + NE; a.arr_zb2 = n_part + NE + 1;   // zbar2 (fp32): absent in lean mode
     a.lean = lean ? 1 : 0;
     a.zb2h = lean ? tc->sig16 + tc->dwl_stride * L : nullptr;
-    if (lean) a.wide = 1;
     for (int i = 0; i < TC_MAX_EH * TC_H / 2; ++i) {      // pair i = (direction, octave) of internal columns 2i, 2i+1
       a.pair_d[i] = (uint8_t)(i < pe_half ? i / lay.n_freqs : 0);
       a.pair_f[i] = (uint8_t)(i < pe_half ? i % lay.n_freqs : 0);
@@ -300,6 +298,8 @@ int tc_forward(isdfb_ctx* ctx, const float* x, const float* noise, float noise_s
 // K2 over the dim^3 lattice of get_sdf_grid with the query points generated in the kernel (no [dim^3, 3] array in HBM)
 int tc_forward_grid(isdfb_ctx* ctx, const float* lin, int dim, const float* scale, const float* transform, float* sdf,
                     cudaStream_t st) {
+  if ((int64_t)dim * dim * dim >= (1LL << 32))       // the chain kernel decodes lattice indices in 32 bits
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "grid dim %d too large for the tensor-core path (dim^3 must be < 2^32)", dim);
   TcGrid g;
   memset(&g, 0, sizeof(g));
   g.lin = lin; g.dim = dim;
@@ -319,6 +319,8 @@ int tc_train(isdfb_ctx* ctx, const float* pc, const float* z_vals, const float* 
              float* loss_sums, cudaStream_t st) {
   TcState* tc = reinterpret_cast<TcState*>(ctx->tc);
   const int64_t n = n_rays * S;
+  if (n >= (1LL << 32))                               // the chain kernel decodes sample indices in 32 bits
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "%lld samples per step exceed the tensor-core path's 2^32", (long long)n);
   const bool two_wave_ok = !tc->profiling && !getenv("ISDFB_NO_OVERLAP");
   // weight-gradient launches of this step as (grid, tiles): with a gradient exchange installed the last CTA of
   // each job over ALL of them forwards the job's tile to the multicast buffer, so it must know how many arrive

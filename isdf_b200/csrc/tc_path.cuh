@@ -25,7 +25,7 @@ struct TcDwArgs {
   int32_t skip_ylo;        // experiment: drop the X_hi*Y_lo pass (Y = layer inputs rounded to bf16)
   const uint8_t *dwl_hi, *dwl_lo;
   size_t dwl_stride;
-  float* g_packed;         // where the TMEM accumulators are flushed (red.global.add): the gradient itself, or with an
+  float* g_packed;         // where the register accumulators are flushed (red.global.add): the gradient itself, or with an
                            // exchange installed the LOCAL staging buffer
   int32_t g_mc;            // 1: exchange installed -- the last CTA of every job forwards the job's finished tile
   float* g_mc_out;         //    from the staging buffer to this MULTICAST address (multimem.red) and clears the stage

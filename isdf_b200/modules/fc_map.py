@@ -119,7 +119,7 @@ class SDFMap(nn.Module):
             except _lib.IsdfbError as e:
                 if self.precision == "fp32" or "tensor-core path supports" not in str(e):
                     raise
-                # shapes the tcgen05 kernels do not take run on the CUDA-core fp32 kernels of the same library
+                # shapes the tensor-core (wgmma) kernels do not take run on the CUDA-core fp32 kernels of the same library
                 warnings.warn("isdf_b200: %s -- using precision 'fp32' (CUDA-core kernels) for this model" % e)
                 self._engine = Engine(dev, pe.n_freqs, self.hidden_size, self.hidden_layers_block, pe.scale,
                                       self.scale_output, transform=pe.transform, precision="fp32",

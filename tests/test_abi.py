@@ -44,9 +44,9 @@ def test_ctypes_binding_covers_header(built):
         assert hasattr(lib, name)
 
 
-def test_sass_is_sm100a(built):
+def test_sass_is_sm90a(built):
     out = subprocess.run(["cuobjdump", "-lelf", built], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_product_does_not_import_oracle():

@@ -1,7 +1,7 @@
 """GPU parity at the model shapes of the other shipped / BASELINE configs (SURVEY.md appendix A): wide MLP 512x(4+4)
 (BASELINE configs[4]), realsense E = 381 (n_embed_funcs 8), franka E = 465 with hidden_layers_block 3.  All three on the
-CUDA-core fp32 path; the two wide embeddings also on the tcgen05 path (two embedding halves); hidden = 512 must be refused
-loudly by the tcgen05 path.  Checked against the fp64 oracle like the default shape.  (File name sorts last on purpose: the default-shape suites
+CUDA-core fp32 path; the two wide embeddings also on the tensor-core path (two embedding halves); hidden = 512 must be refused
+loudly by the tensor-core path.  Checked against the fp64 oracle like the default shape.  (File name sorts last on purpose: the default-shape suites
 run first.)"""
 import pytest
 import torch
@@ -52,7 +52,7 @@ def test_fp32_path_matches_oracle_at_other_shapes(tag, n_freqs, hidden, block):
 @pytest.mark.parametrize("mode", ["bf16x3", "bf16x3g"])
 @pytest.mark.parametrize("tag,n_freqs,hidden,block", SHAPES[1:], ids=[s[0] for s in SHAPES[1:]])
 def test_tensor_core_path_wide_embeddings_match_oracle(tag, n_freqs, hidden, block, mode):
-    """E = 381 / 465 (n_embed_funcs 8 / 10 of the realsense / franka configs, block 3) on the tcgen05 path: the padded
+    """E = 381 / 465 (n_embed_funcs 8 / 10 of the realsense / franka configs, block 3) on the tensor-core path: the padded
     embedding is two halves of 256 internal columns, every embedding-fed product the sum of two 128x256x256 products."""
     cfg, sd, batch, noise = _case(n_freqs, hidden, block, R=60, S=16)          # 960 samples: 8 tiles, 2 chunks
     eng = P.make_engine(DEV, cfg, mode, max_points=512)

@@ -174,21 +174,25 @@ def test_scannet_reader_and_intrinsics(tmp_path):
     assert np.allclose(s["T"], C.synthetic_pose(2).numpy())
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/isdf"), reason="needs the reference checkout (build container only)")
 def test_alias_package_layers_over_the_reference_checkout():
     """INTEGRATION.md section 1: with this repo BEFORE the reference on sys.path, the drivers' imports resolve --
-    replaced modules here, everything else (isdf.visualisation, isdf.eval.plot_utils, missing names) in the reference."""
+    replaced modules here, everything else (isdf.visualisation, isdf.eval.plot_utils, missing names) in the reference
+    (the checkout, or the verbatim copy build() leaves under oracle/_ref)."""
     import subprocess
     import sys
+    from oracle import make_ref, ref_shim
+    if not ref_shim.available():
+        assert make_ref.populate(), "neither the reference checkout nor oracle/_ref is present: run build()"
+    ref = ref_shim.REFERENCE_ROOT
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     res = subprocess.run([sys.executable, os.path.join(root, "tools", "dropin_check.py")], capture_output=True, text=True,
                          timeout=300)
     assert res.returncode == 0, res.stdout + res.stderr
     out = res.stdout
     assert "trainer from %s" % os.path.join(root, "isdf_b200", "modules", "trainer.py") in out
-    assert "visualisation from /root/reference/isdf/visualisation/__init__.py" in out
+    assert "visualisation from %s" % os.path.join(ref, "isdf", "visualisation", "__init__.py") in out
     assert "accuracy_comp (fallback): isdf_reference.eval.metrics" in out
-    assert "isdf.eval.plot_utils from /root/reference/isdf/eval/plot_utils.py" in out
+    assert "isdf.eval.plot_utils from %s" % os.path.join(ref, "isdf", "eval", "plot_utils.py") in out
 
 
 def test_reference_copy_is_verbatim_and_steps_on_cpu(tmp_path):

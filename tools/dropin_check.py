@@ -1,6 +1,7 @@
 import sys
-import os; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__)))); sys.path.append(os.environ.get('ISDF_REFERENCE', '/root/reference'))
+import os; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import ref_shim
+sys.path.append(ref_shim.REFERENCE_ROOT)               # the reference checkout, or its verbatim copy under oracle/_ref
 sys.meta_path.insert(0, ref_shim._MockFinder())        # GUI / mesh libraries are absent in this container
 import isdf
 from isdf import visualisation
