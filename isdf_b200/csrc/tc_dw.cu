@@ -114,7 +114,7 @@ __global__ void __launch_bounds__(DW_THREADS, 1) tc_dw_kernel(const __grid_const
             wgmma_m64n256k16<1, 1>(d_main, ah, bh, acc_main);
             if (kPasses == 3) {
               wgmma_m64n256k16<1, 1>(d_main, al, bh, 1);
-              if (!args.skip_ylo) wgmma_m64n256k16<1, 1>(d_main, ah, gmma_desc(base + Cfg::kXBytes + 8192, 128, 256), 1);
+              wgmma_m64n256k16<1, 1>(d_main, ah, gmma_desc(base + Cfg::kXBytes + 8192, 128, 256), 1);
             }
             acc_main = 1;
           }

@@ -1,7 +1,6 @@
 // Host orchestration of the tensor-core path: state, step programs, weight-gradient jobs, launches.
 #include "tc_path.cuh"
 #include <new>
-#include <stdlib.h>
 
 static TcStep& add_step(TcChainArgs& a, int unit, int orient, int epi, int layer, int aux = 0) {
   TcStep& s = a.steps[a.n_steps++];
@@ -61,12 +60,6 @@ static void build_program(const ModelLayout& lay, int mode, int NE, TcChainArgs&
   }
   // ---- S4 (reverse; the two d / d e products are not needed)
   for (int l = L - 1; l >= 1; --l) add_step(a, l, 1, EPI_S4, l - 1);
-  if (getenv("ISDFB_GRAD_2PASS"))          // experiment: weights as single bf16 in the gradient-only sweeps
-    for (int s = 0; s < a.n_steps; ++s)
-      if (a.steps[s].epi == EPI_S3 || a.steps[s].epi == EPI_S3_LAST || a.steps[s].epi == EPI_S4 ||
-          (a.steps[s].epi == EPI_RAW && a.steps[s].aux != PART_CAT_S1 && a.steps[s].aux != PART_CAT_S2 &&
-           a.steps[s].aux != PART_CAT_S2_H1 && a.steps[s].aux != PART_L0_S1))
-        a.steps[s].flags |= STF_NO_BLO;
 }
 
 // Host-only view of the step program (no CUDA call, no context): what the chain kernel will run for a model shape.
@@ -168,20 +161,12 @@ int tc_create(isdfb_ctx* ctx) {
 
   ISDFB_CUDA_OK(ctx, cudaMalloc(&tc->dw_counters, TC_MAX_JOBS * sizeof(int32_t)));
   ISDFB_CUDA_OK(ctx, cudaMemset(tc->dw_counters, 0, TC_MAX_JOBS * sizeof(int32_t)));
-  if (getenv("ISDFB_DEBUG_CLOCK")) {
-    ISDFB_CUDA_OK(ctx, cudaMalloc(&tc->dbg_clock, 128 * sizeof(long long)));
-    ISDFB_CUDA_OK(ctx, cudaMemset(tc->dbg_clock, 0, 128 * sizeof(long long)));
-  }
   for (int mode = 0; mode < 3; ++mode) {
     TcChainArgs& a = tc->proto[mode];
     memset(&a, 0, sizeof(a));
     build_program(lay, mode, NE, a);
     a.n_eh = NE;
     a.mode = mode; a.L = L; a.ic = ic; a.E = lay.E;
-    a.prefetch = getenv("ISDFB_NO_PREFETCH") ? 0 : 1;
-    a.stagger = getenv("ISDFB_STAGGER") ? atoi(getenv("ISDFB_STAGGER")) : 1;
-    a.ablate = getenv("ISDFB_ABLATE") ? atoi(getenv("ISDFB_ABLATE")) : 0;
-    a.dbg_clock = tc->dbg_clock;
     a.pe = ctx->pe;
     a.scale_output = ctx->cfg.scale_output;
     a.w_img = tc->w_img;
@@ -241,7 +226,6 @@ int tc_create(isdfb_ctx* ctx) {
   d.g_packed = ctx->g_packed;
   d.wout_off = lay.wout_off;
   d.scale_output = ctx->cfg.scale_output;
-  d.skip_ylo = getenv("ISDFB_DW_SKIP_YLO") ? 1 : 0;
   return ISDFB_OK;
 }
 
@@ -321,7 +305,7 @@ int tc_train(isdfb_ctx* ctx, const float* pc, const float* z_vals, const float* 
   const int64_t n = n_rays * S;
   if (n >= (1LL << 32))                               // the chain kernel decodes sample indices in 32 bits
     ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "%lld samples per step exceed the tensor-core path's 2^32", (long long)n);
-  const bool two_wave_ok = !tc->profiling && !getenv("ISDFB_NO_OVERLAP");
+  const bool two_wave_ok = !tc->profiling;
   // weight-gradient launches of this step as (grid, tiles): with a gradient exchange installed the last CTA of
   // each job over ALL of them forwards the job's tile to the multicast buffer, so it must know how many arrive
   int32_t expect[TC_MAX_JOBS] = {0};
@@ -414,14 +398,6 @@ extern "C" int isdfb_debug_buffers(isdfb_ctx* ctx, float** aux, int64_t* aux_str
   *aux = tc->aux; *aux_stride_floats = (int64_t)tc->aux_stride;
   *dwl_hi = tc->dwl_hi; *dwl_lo = tc->dwl_lo; *dwl_stride_bytes = (int64_t)tc->dwl_stride;
   *n_aux = tc->n_aux; *n_dwl = tc->n_dwl; *tiles_cap = tc->tiles_cap; *sig16 = tc->sig16;
-  if (tc->dbg_clock) {   // debug timeline: printed by the host on request
-    long long h[128];
-    cudaMemcpy(h, tc->dbg_clock, sizeof(h), cudaMemcpyDeviceToHost);
-    const int ns = tc->proto[TC_MODE_TRAIN].n_steps;
-    printf("[isdfb] CTA0 tile0 timeline (cycles): PE took %lld; PE_end=0", h[0] - h[120]);
-    for (int s = 0; s < ns; ++s) printf(" | s%d epi%d wait_end=%lld epi_end=%lld", s, tc->proto[TC_MODE_TRAIN].steps[s].epi, h[1 + 2 * s] - h[0], h[2 + 2 * s] - h[0]);
-    printf("\n");
-  }
   return ISDFB_OK;
 }
 

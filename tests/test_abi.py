@@ -58,6 +58,15 @@ def test_product_does_not_import_oracle():
                 assert "oracle" not in txt or "import oracle" not in txt and "from oracle" not in txt, f
 
 
+def test_native_code_reads_no_environment_switches():
+    """What the library computes and how it launches depends on its arguments only: no kernel or host source reads the
+    environment, and there is no build-time variant of the kernels."""
+    csrc = os.path.join(ROOT, "isdf_b200", "csrc")
+    for f in sorted(os.listdir(csrc)):
+        txt = open(os.path.join(csrc, f)).read()
+        assert "getenv" not in txt and not re.search(r"\bISDFB_DEV_\w+", txt), f
+
+
 def test_no_cpu_fallback():
     import torch
     from isdf_b200.engine import Engine
