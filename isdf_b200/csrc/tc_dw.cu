@@ -221,6 +221,9 @@ __global__ void __launch_bounds__(DW_THREADS, 1) tc_dw_kernel(const __grid_const
 }
 
 int tc_dw_launch(isdfb_ctx* ctx, const TcDwArgs& args, int passes, int grid, cudaStream_t st) {
+  if (grid < args.n_jobs)          // CTA b runs job b % n_jobs: with fewer CTAs, jobs grid..n_jobs-1 would be skipped
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "weight-gradient launch of %d CTAs for %d jobs: every job needs a CTA", grid,
+               args.n_jobs);
   if (passes == 3) {
     tc_dw_kernel<3><<<grid, DW_THREADS, DwCfg<3>::kSmem, st>>>(args);
   } else {

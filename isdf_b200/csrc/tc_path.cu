@@ -250,6 +250,13 @@ static inline int passes_of(const isdfb_ctx* ctx) {
 // the weight-gradient kernel reads single-bf16 operands in lean mode
 static inline int dw_passes_of(const isdfb_ctx* ctx) { return ctx->cfg.precision == ISDFB_PREC_BF16X3 ? 3 : 1; }
 
+// Grid of the two-wave plan's wave-1 weight-gradient launch: the SMs that wave 2 (rest tiles) leaves free, but at
+// least one CTA per job -- tc_dw_kernel gives CTA b the job b % n_jobs, so a smaller grid would skip whole jobs.
+static inline int wave1_dw_grid(const TcState* tc, int rest) {
+  const int free_sms = tc->num_sms - rest;
+  return free_sms > tc->dw.n_jobs ? free_sms : tc->dw.n_jobs;
+}
+
 static int tc_forward_impl(isdfb_ctx* ctx, const float* x, const float* noise, float noise_std, int64_t n, float* sdf,
                            float* grad, cudaStream_t st, const TcGrid* grid) {
   TcState* tc = reinterpret_cast<TcState*>(ctx->tc);
@@ -321,7 +328,7 @@ int tc_train(isdfb_ctx* ctx, const float* pc, const float* z_vals, const float* 
       const int tiles = (int)((nc + TC_TILE - 1) / TC_TILE);
       if (tiles > tc->num_sms && tiles < 2 * tc->num_sms && two_wave_ok) {
         const int rest = tiles - tc->num_sms;
-        plan(tc->num_sms - rest > 14 ? tc->num_sms - rest : 14, tc->num_sms);
+        plan(wave1_dw_grid(tc, rest), tc->num_sms);
         plan(tc->num_sms, rest);
       } else {
         plan(tc->num_sms, tiles);
@@ -365,7 +372,7 @@ int tc_train(isdfb_ctx* ctx, const float* pc, const float* z_vals, const float* 
       ISDFB_CUDA_OK(ctx, cudaStreamWaitEvent(tc->side, tc->ev_fork, 0));
       d.tile0 = 0; d.n_tiles = tc->num_sms;
       const int rest = total_tiles - tc->num_sms;
-      rc = tc_dw_launch(ctx, d, dw_passes_of(ctx), tc->num_sms - rest > 14 ? tc->num_sms - rest : 14, tc->side);
+      rc = tc_dw_launch(ctx, d, dw_passes_of(ctx), wave1_dw_grid(tc, rest), tc->side);
       if (rc) return rc;
       ISDFB_CUDA_OK(ctx, cudaEventRecord(tc->ev_join, tc->side));
       a.tile0 = tc->num_sms; a.n_tiles = rest;
