@@ -216,7 +216,7 @@ int isdfb_frame_bins(isdfb_ctx* ctx, const float* loss_mat, const uint8_t* ray_v
                      int32_t n_samples, int32_t n_frames, int32_t H, int32_t W, int32_t factor,
                      float* loss_approx, float* frame_avg, void* stream);
 
-/* K5 + the step's bookkeeping in the same launches (the graphed fast-mode step): as isdfb_frame_bins, plus
+/* K5 + the step's bookkeeping in the same launches (Trainer.step in every mode): as isdfb_frame_bins, plus
  *   frame_avg_losses[frame_map[f]] = frame_avg[f]      -- trainer.py:979 `frames.frame_avg_losses[idxs] = ...`
  *   means_out[i] = loss_sums[i] * inv_count[0], i < 4  -- the loss means the reference reads with .item()
  *                                                          (loss.py:187-203); loss_sums is then CLEARED, so the next

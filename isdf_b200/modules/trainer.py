@@ -7,7 +7,7 @@ sample_points / sdf_eval_and_loss.  One step launches (reference trainer.py:951-
 
     K1 isdfb_gather_rays + isdfb_sample_rays      (sample.py, transform.py)
     K4 isdfb_train_fwd_bwd                        (embedding.py, fc_map.py, loss.py, backward())
-    K5 isdfb_frame_bins                           (loss.frame_avg)
+    K5 isdfb_step_finish                          (loss.frame_avg + the write-back + the loss means)
     C1 one NCCL all-reduce of the flat gradient   (new: data-parallel keyframe shards)
     K6 isdfb_adamw                                (optim.AdamW.step + weight re-pack)
 
@@ -139,8 +139,6 @@ class Trainer:
         self.fix_normal_window = bool(b200.get("fix_normal_window", 0))
         self.max_points = int(b200.get("max_points", 32768))
         self.use_graph = bool(b200.get("cuda_graph", 1))
-        # fast mode: K1 fused sampler with in-kernel Philox numbers (one launch instead of ~10 torch kernels)
-        self.fused_sampler = bool(b200.get("fused_sampler", int(os.environ.get("ISDFB_FUSED_SAMPLER", "1"))))
         self._sampler_seed = None
         self._graph = None
         self._graph_seen = None
@@ -173,9 +171,8 @@ class Trainer:
             self.load_checkpoint(chkpt_load_file)
         self.sdf_map.train()
         self.cosSim = torch.nn.CosineSimilarity(dim=-1, eps=1e-6)
+        # the step's K4 accumulates into these sums; the step's isdfb_step_finish clears them again
         self._loss_sums = torch.zeros(4, dtype=torch.float32, device=self.device)
-        self._loss_sums_fused = torch.zeros(4, dtype=torch.float32, device=self.device)
-        self._means_dev = torch.zeros(4, dtype=torch.float32, device=self.device)
         self._arange_cache = {}
         self._last_pts = None
         self._t_events = None
@@ -501,6 +498,16 @@ class Trainer:
         return [*rand_ints, n - 2, n - 1]
 
     # ---- sampling (trainer.py:683-766) -------------------------------------------------------
+    def _fused_sampling(self, n_surf):
+        """Fast mode samples with in-kernel Philox numbers unless torch's generator on rng_device is asked for, or
+        there are no surface samples."""
+        return self.rng_mode == "fast" and self.rng_device is None and n_surf >= 1
+
+    def _philox_seed(self):
+        if self._sampler_seed is None:            # one draw from torch's generator seeds the in-kernel streams
+            self._sampler_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        return self._sampler_seed
+
     def _lin(self, n):
         if n not in self._lin_cache:
             self._lin_cache[n] = torch.linspace(0, 1, n + 1).to(self.device)
@@ -519,13 +526,11 @@ class Trainer:
         eng = self.sdf_map.engine()
         dev = self.device
         n_frames = depth_batch.shape[0] if frame_map is None else len(frame_map)
-        if self.rng_mode == "fast" and self.fused_sampler and n_surf >= 1 and self.rng_device is None:
-            if self._sampler_seed is None:            # one draw from torch's generator seeds the in-kernel stream
-                self._sampler_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        if self._fused_sampling(n_surf):
             fmap = None if frame_map is None else torch.as_tensor(frame_map, device=dev, dtype=torch.int64)
             out = eng.sample_fused(depth_batch, norm_batch, T_WC_batch, fmap, n_frames, n_rays, n_strat, n_surf,
-                                   self.cam, self.min_depth, dist_behind_surf, self._lin(n_strat), self._sampler_seed,
-                                   want_noise=True, normals_use_frame_map=self.fix_normal_window)
+                                   self.cam, self.min_depth, dist_behind_surf, self._lin(n_strat), self._philox_seed(),
+                                   want_noise=self.noise_std is not None, normals_use_frame_map=self.fix_normal_window)
             out.update(depth_batch=depth_batch, binary_masks=None, n_frames=n_frames)
             return out
         rd = self.rng_device or dev
@@ -559,49 +564,59 @@ class Trainer:
         """K4 (+K5).  Returns (total_loss, losses, loss_approx, frame_avg_loss) like the reference;
         the parameter gradient of total_loss is left in the engine's gradient buffer (the fused
         kernel already did the double back-prop), so no .backward() follows."""
+        # K4 accumulates into fresh sums, so the step's buffer stays cleared for the next step
+        sums, loss_mat, inv_count, _ = self._train_batch(sample_pts, zero_grad, loss_sums=None)
+        losses = self._report(sums * inv_count)
+        loss_approx = frame_avg_loss = None
+        if do_avg_loss:
+            loss_approx, frame_avg_loss = self.sdf_map.engine().frame_bins(
+                loss_mat, sample_pts["indices_b"], sample_pts["indices_h"], sample_pts["indices_w"],
+                sample_pts["n_frames"], self.H, self.W, self.loss_approx_factor, ray_valid=sample_pts.get("ray_valid"))
+        return losses["total_loss"], losses, loss_approx, frame_avg_loss
+
+    def _train_batch(self, pts, zero_grad, loss_sums):
+        """[bounds 'pc'] + K4 on a sampled batch: the noise, 1 / (valid rays * S) and the loss config around
+        isdfb_train_fwd_bwd.  Returns (loss sums, loss_mat, 1 / (valid rays * S) as a one-element device tensor,
+        (the batch with its noise, the loss config))."""
         if self.bounds_method == "normal":
             raise TypeError("bounds_method 'normal' is broken in the reference itself (loss.py:29 calls "
                             "bounds_ray with 3 of its 5 arguments) and is not supported")
         eng = self.sdf_map.engine()
-        pc = sample_pts["pc"]
+        pc = pts["pc"]
         R, S = pc.shape[0], pc.shape[1]
-        ray_valid = sample_pts.get("ray_valid")
+        ray_valid = pts.get("ray_valid")
         pc_bounds = pc_vec = None
         if self.bounds_method == "pc":          # N2: all-pairs batch-distance bound (loss.py:56-89)
-            pc_bounds, pc_vec = eng.bounds_pc(pc, sample_pts["z_vals"], sample_pts["depth_sample"],
-                                              ray_valid=ray_valid)
+            pc_bounds, pc_vec = eng.bounds_pc(pc, pts["z_vals"], pts["depth_sample"], ray_valid=ray_valid)
         noise = None
         if self.noise_std is not None:
-            noise = sample_pts.get("noise")           # drawn by the fused sampler, else here (fc_map.py:106-108)
+            noise = pts.get("noise")           # drawn by the fused sampler, else here (fc_map.py:106-108)
             if noise is None:
                 noise = torch.randn(R, S, device=self.rng_device or self.device).to(self.device)
-        inv_dev = sample_pts.get("inv_count_dev")     # 1 / (valid rays * S), computed by the fused sampler
-        if inv_dev is not None:
-            inv_count = 0.0
-        elif ray_valid is None:
+        inv_count, inv_dev = 0.0, pts.get("inv_count_dev")      # computed by the fused sampler
+        if inv_dev is None and ray_valid is None:
             inv_count = 1.0 / max(R * S, 1)
-        else:
-            inv_count = 0.0
+        elif inv_dev is None:
             cnt = ray_valid.sum().float() * S
             inv_dev = (1.0 / cnt.clamp_min(1.0)).reshape(1)
         lc = make_loss_cfg(self.trunc_weight, self.trunc_distance, self.eik_weight, self.eik_apply_dist,
                            self.grad_weight, self.orien_loss, self.loss_type, self.noise_std or 0.0, inv_count,
                            inv_count_dev=inv_dev, bounds=pc_bounds, grad_vec=pc_vec)
-        self._loss_sums.zero_()
         if zero_grad:
             eng.zero_grad()
-        sdf, _, loss_mat, sums = eng.train_fwd_bwd(pc, sample_pts["z_vals"], sample_pts["depth_sample"],
-                                                   sample_pts["dirs_C_sample"], sample_pts["T_WC_sample"],
-                                                   sample_pts["norm_sample"] if self.do_normal else None, noise, lc,
-                                                   ray_valid=ray_valid, want_grad=False, loss_sums=self._loss_sums)
-        means = sums * (inv_dev if inv_dev is not None else inv_count)
+        sdf, _, loss_mat, sums = eng.train_fwd_bwd(pc, pts["z_vals"], pts["depth_sample"], pts["dirs_C_sample"],
+                                                   pts["T_WC_sample"], pts["norm_sample"] if self.do_normal else None,
+                                                   noise, lc, ray_valid=ray_valid, want_grad=False, loss_sums=loss_sums)
+        self.last_sdf, self.last_loss_mat = sdf, loss_mat
+        if inv_dev is None:
+            # K4 read inv_count as fp32 (LossCfg); the loss means multiply by the same fp32 value
+            inv_dev = torch.full((1,), inv_count, dtype=torch.float32, device=self.device)
+        return sums, loss_mat, inv_dev, (dict(pts, noise=noise), lc)
+
+    def _report(self, means):
+        """The four loss means [sdf, grad, eikonal, total] -> the losses dict of step()."""
         if self.rng_mode == "reference":
             host = means.tolist()                                  # the reference's 3 .item() syncs, in one
-            losses = {"sdf_loss": host[0]}
-            if self.grad_weight != 0:
-                losses["grad_loss"] = host[1]
-            if self.eik_weight != 0:
-                losses["eikonal_loss"] = host[2]
             total_loss = means[3]
         else:
             # fast mode: the four means are delivered to pinned host memory by the step itself (an async D2H
@@ -612,104 +627,57 @@ class Trainer:
                 self._loss_host = torch.zeros(4, dtype=torch.float32).pin_memory()
             self._loss_host.copy_(means, non_blocking=True)
             host = self._loss_host
-            losses = {"sdf_loss": host[0]}
-            if self.grad_weight != 0:
-                losses["grad_loss"] = host[1]
-            if self.eik_weight != 0:
-                losses["eikonal_loss"] = host[2]
             total_loss = host[3]
-        losses["total_loss"] = total_loss
-        self.last_sdf, self.last_loss_mat = sdf, loss_mat
-        loss_approx = frame_avg_loss = None
-        if do_avg_loss:
-            loss_approx, frame_avg_loss = eng.frame_bins(loss_mat, sample_pts["indices_b"], sample_pts["indices_h"],
-                                                         sample_pts["indices_w"], sample_pts["n_frames"], self.H,
-                                                         self.W, self.loss_approx_factor, ray_valid=ray_valid)
-        return total_loss, losses, loss_approx, frame_avg_loss
-
-    # ---- one optimisation step (trainer.py:951-1016) -----------------------------------------
-    def _fused_front_ok(self):
-        return (self.rng_mode == "fast" and self.fused_sampler and self.rng_device is None and self.n_surf_samples >= 1
-                and self.window_size <= 66)
-
-    def _step_front_fused(self, zero_grad=True):
-        """fast mode, all on the device and all in this library's kernels: window (A0, Gumbel top-k) -> fused sampler
-        (A1-A3 + the noise draw) -> [bounds 'pc'] -> K4 -> K5 + write-back of the per-keyframe losses + loss means.
-        No torch kernel is launched; the only torch node of a captured step is the 16-byte D2H copy of the means."""
-        eng = self.sdf_map.engine()
-        f = self.frames
-        n = len(f)
-        dev = self.device
-        if self._sampler_seed is None:            # one draw from torch's generator seeds the in-kernel streams
-            self._sampler_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        if n > self.window_size and self.incremental:
-            fmap = eng.select_window(f.frame_avg_losses, n, self.window_size, self._sampler_seed)
-        else:
-            fmap = self._arange_cache.get(n)
-            if fmap is None:
-                fmap = self._arange_cache[n] = torch.arange(n, device=dev, dtype=torch.int64)
-        self.active_idxs = fmap
-        n_win = int(fmap.shape[0])
-        norm_batch = f.normal_batch if self.do_normal else None
-        pts = eng.sample_fused(f.depth_batch, norm_batch, f.T_WC_batch, fmap, n_win, self.n_rays,
-                               self.n_strat_samples, self.n_surf_samples, self.cam, self.min_depth,
-                               self.dist_behind_surf, self._lin(self.n_strat_samples), self._sampler_seed,
-                               want_noise=self.noise_std is not None, normals_use_frame_map=self.fix_normal_window)
-        self.active_pixels = {k: pts[k] for k in ("indices_b", "indices_h", "indices_w")}
-        if self.bounds_method == "normal":
-            raise TypeError("bounds_method 'normal' is broken in the reference itself (loss.py:29) and is not supported")
-        pc_bounds = pc_vec = None
-        if self.bounds_method == "pc":
-            pc_bounds, pc_vec = eng.bounds_pc(pts["pc"], pts["z_vals"], pts["depth_sample"], ray_valid=pts["ray_valid"])
-        inv_dev = pts["inv_count_dev"]
-        lc = make_loss_cfg(self.trunc_weight, self.trunc_distance, self.eik_weight, self.eik_apply_dist,
-                           self.grad_weight, self.orien_loss, self.loss_type, self.noise_std or 0.0, 0.0,
-                           inv_count_dev=inv_dev, bounds=pc_bounds, grad_vec=pc_vec)
-        if zero_grad:
-            eng.zero_grad()
-        # loss_sums is cleared by the previous step's isdfb_step_finish (and at allocation)
-        sdf, _, loss_mat, _ = eng.train_fwd_bwd(pts["pc"], pts["z_vals"], pts["depth_sample"], pts["dirs_C_sample"],
-                                                pts["T_WC_sample"], pts["norm_sample"] if self.do_normal else None,
-                                                pts["noise"], lc, ray_valid=pts["ray_valid"], want_grad=False,
-                                                loss_sums=self._loss_sums_fused)
-        self.last_sdf, self.last_loss_mat = sdf, loss_mat
-        self._last_pts = (pts, lc)            # the step's batch (kept for diagnostics: bench.py re-runs K4 on it)
-        eng.step_finish(loss_mat, pts["indices_b"], pts["indices_h"], pts["indices_w"], n_win, self.H, self.W,
-                        self.loss_approx_factor, pts["ray_valid"], fmap, f.frame_avg_losses, self._loss_sums_fused,
-                        inv_dev, self._means_dev)
-        if self._loss_host is None:
-            self._loss_host = torch.zeros(4, dtype=torch.float32).pin_memory()
-        self._loss_host.copy_(self._means_dev, non_blocking=True)
-        host = self._loss_host
         losses = {"sdf_loss": host[0]}
         if self.grad_weight != 0:
             losses["grad_loss"] = host[1]
         if self.eik_weight != 0:
             losses["eikonal_loss"] = host[2]
-        losses["total_loss"] = host[3]
+        losses["total_loss"] = total_loss
         return losses
 
-    def _step_front(self, zero_grad=True):
-        """Everything up to and including the fused forward/backward (gradient left in the engine)."""
-        if self._fused_front_ok():
-            return self._step_front_fused(zero_grad=zero_grad)
-        depth_batch = self.frames.depth_batch
-        T_WC_batch = self.frames.T_WC_batch
-        norm_batch = self.frames.normal_batch if self.do_normal else None
-        if len(self.frames) > self.window_size and self.incremental:
+    # ---- one optimisation step (trainer.py:951-1016) -----------------------------------------
+    def _window(self):
+        """The step's keyframe window: (active_idxs, the same as an int64 device tensor).  The device draw (A0, at most
+        66 frames) runs only in front of the fused sampler: it reads the Philox step counter that only the fused
+        sampler advances, so without it every step would draw the same window."""
+        n = len(self.frames)
+        if n > self.window_size and self.incremental:
+            if self._fused_sampling(self.n_surf_samples) and self.window_size <= 66:
+                fmap = self.sdf_map.engine().select_window(self.frames.frame_avg_losses, n, self.window_size,
+                                                           self._philox_seed())
+                return fmap, fmap
             idxs = self.select_keyframes()
         elif self.rng_mode == "fast":
-            idxs = torch.arange(T_WC_batch.shape[0], device=self.device)
+            idxs = self._arange_cache.get(n)
+            if idxs is None:
+                idxs = self._arange_cache[n] = torch.arange(n, device=self.device, dtype=torch.int64)
         else:
-            idxs = np.arange(T_WC_batch.shape[0])
-        self.active_idxs = idxs
-        idx_t = idxs if torch.is_tensor(idxs) else torch.as_tensor(idxs, device=self.device, dtype=torch.int64)
-        sample_pts = self.sample_points(depth_batch, T_WC_batch, norm_batch=norm_batch, frame_map=idx_t)
-        self.active_pixels = {k: sample_pts[k] for k in ("indices_b", "indices_h", "indices_w")}
-        total_loss, losses, active_loss_approx, frame_avg_loss = self.sdf_eval_and_loss(sample_pts, do_avg_loss=True,
-                                                                                        zero_grad=zero_grad)
-        self.frames.frame_avg_losses[idx_t] = frame_avg_loss
-        return losses
+            idxs = np.arange(n)
+        return idxs, idxs if torch.is_tensor(idxs) else torch.as_tensor(idxs, device=self.device, dtype=torch.int64)
+
+    def _step_front(self, zero_grad=True):
+        """Everything up to and including the fused forward/backward (gradient left in the engine): window -> K1 ->
+        [bounds 'pc'] + K4 -> K5 with the write-back of the per-keyframe losses and the loss means."""
+        f = self.frames
+        self.active_idxs, fmap = self._window()
+        pts = self.sample_points(f.depth_batch, f.T_WC_batch, norm_batch=f.normal_batch if self.do_normal else None,
+                                 frame_map=fmap)
+        self.active_pixels = {k: pts[k] for k in ("indices_b", "indices_h", "indices_w")}
+        means = torch.empty(4, dtype=torch.float32, device=self.device)
+        # _last_pts keeps the step's batch and loss config for diagnostics (bench.py re-runs K4 on it)
+        try:
+            sums, loss_mat, inv_count, self._last_pts = self._train_batch(pts, zero_grad, self._loss_sums)
+            # clears the sums K4 accumulated, so the next step's K4 starts from zero
+            self.sdf_map.engine().step_finish(loss_mat, pts["indices_b"], pts["indices_h"], pts["indices_w"],
+                                              pts["n_frames"], self.H, self.W, self.loss_approx_factor,
+                                              pts["ray_valid"], fmap, f.frame_avg_losses, sums, inv_count, means)
+        except Exception:
+            # K4 may have accumulated without a step_finish to clear it; a failed capture launched nothing
+            if not torch.cuda.is_current_stream_capturing():
+                self._loss_sums.zero_()
+            raise
+        return self._report(means)
 
     def _allreduce(self):
         """C1 (NCCL form): the only collective -- sum of the packed gradient over the data-parallel ranks."""
