@@ -12,7 +12,9 @@
  *   - all data pointers are caller-owned DEVICE pointers (torch storage) unless the name
  *     says `host`; fp32 unless stated; indices are int64 as in the reference;
  *   - `stream` is a cudaStream_t passed as void*; nothing synchronises the device, nothing
- *     allocates after isdfb_create (workspaces are sized by max_points);
+ *     allocates after isdfb_create (workspaces are sized by max_points) -- except the lattice- and
+ *     mesh-sized workspaces of the mesh entries, which grow on first use, and whose count calls
+ *     wait for their stream to return the sizes;
  *   - calls may come from any host thread (train_vis.py steps from a worker thread):
  *     every call does cudaSetDevice(ctx->device) itself.
  */
@@ -264,6 +266,47 @@ int isdfb_set_grad_exchange(isdfb_ctx* ctx, float* local0, float* local1, float*
 int isdfb_select_grad_buffer(isdfb_ctx* ctx, int32_t which);
 int isdfb_zero_grad_buffer(isdfb_ctx* ctx, int32_t which, void* stream);
 
+/* ---- N4: mesh extraction (Trainer.mesh_rec / write_mesh, trainer.py:1500-1542) --------------------------------
+ * Marching cubes at level 0 over the lattice isdfb_mlp_forward_grid writes, sdf[(i*dim + j)*dim + k] (axis 0 = box x):
+ * replaces skimage.measure.marching_cubes + the affine map of draw3D.draw_mesh (draw3D.py:111-145).  A value is inside
+ * iff f < 0; one vertex per sign-changing lattice edge (point (i,j,k) owns its +x, +y, +z edges), at p0 + t e with
+ * t = (0 - f0) / (f1 - f0); then u = 2 p / (dim - 1) - 1 and x = T[:3,:3] (s * u) + T[:3,3], s = scale [3] and
+ * T = transform [3x4 row-major] as HOST arrays (NULL = ones / identity), the values get_sdf_grid passes to
+ * isdfb_mlp_forward_grid.  Vertices come in order of the owning lattice point, then edge axis x, y, z; faces in order of
+ * the cube, then the case table; (v1 - v0) x (v2 - v0) points towards increasing SDF.  No atomics: two runs are
+ * bitwise equal.
+ * isdfb_mesh_count classifies the cubes and scans the counts (SYNCHRONOUS: returns the vertex and face counts); 2 <= dim
+ *   <= 2048, more than 2^31 - 1 vertices is ISDFB_ERR_CAPACITY (faces are int32).
+ * isdfb_mesh_emit writes verts [V,3] f32 and faces [F,3] int32 for the lattice of the last count (same sdf pointer and
+ *   dim, else ISDFB_ERR_STATE); cap_verts / cap_faces are the rows the outputs hold, a smaller capacity than the count is
+ *   ISDFB_ERR_CAPACITY and nothing is written.
+ * Workspace: 9 bytes per lattice point, owned by the ctx, grown on demand.                                           */
+int isdfb_mesh_count(isdfb_ctx* ctx, const float* sdf, int32_t dim, int64_t* n_verts /*host*/,
+                     int64_t* n_faces /*host*/, void* stream);
+int isdfb_mesh_emit(isdfb_ctx* ctx, const float* sdf, int32_t dim, const float* scale /*[3], host*/,
+                    const float* transform /*[12], host*/, float* verts, int64_t cap_verts, int32_t* faces,
+                    int64_t cap_faces, void* stream);
+
+/* The crop of mesh_rec (trainer.py:1504-1533, update_vis_vars 1020-1049, transform.py:127-167, draw3D.py:80-108, and the
+ * scipy KD-tree query + trimesh update_faces / remove_unreferenced_vertices that follow).
+ * isdfb_mesh_cloud: every keyframe's depth [F,H,W], nearest-resized to (H_vis, W_vis) as OpenCV INTER_NEAREST (source
+ *   index floor(dst * src / dst)), back-projected with the given (reduced) intrinsics and moved to the world by T_WC
+ *   [F,4,4]: cloud [F*H_vis*W_vis, 3].  Depth 0 lands on the camera centre and stays; NaN depth gives a NaN point that
+ *   the crop drops.  box [6] (device) = min xyz, max xyz of the finite points (NaN if there is none).
+ * isdfb_mesh_crop_count: keeps a vertex iff a finite cloud point is closer than crop_dist (uniform hash grid of cell
+ *   crop_dist, 27 cells per query), a face iff any of its vertices is kept, and the vertices the kept faces reference
+ *   (SYNCHRONOUS: returns the kept counts).  A face index outside [0, n_verts) is ISDFB_ERR_ARG.
+ * isdfb_mesh_crop_emit: the kept vertices and faces, renumbered in order, for the mesh of the last crop count (same
+ *   pointers and sizes, else ISDFB_ERR_STATE); capacity below the count is ISDFB_ERR_CAPACITY.                     */
+int isdfb_mesh_cloud(isdfb_ctx* ctx, const float* depth, const float* T_WC, int32_t n_frames, int32_t H, int32_t W,
+                     int32_t H_vis, int32_t W_vis, float fx, float fy, float cx, float cy, float* cloud, float* box,
+                     void* stream);
+int isdfb_mesh_crop_count(isdfb_ctx* ctx, const float* cloud, int64_t n_cloud, float crop_dist, const float* verts,
+                          int64_t n_verts, const int32_t* faces, int64_t n_faces, int64_t* n_verts_kept /*host*/,
+                          int64_t* n_faces_kept /*host*/, void* stream);
+int isdfb_mesh_crop_emit(isdfb_ctx* ctx, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces,
+                         float* verts_out, int64_t cap_verts, int32_t* faces_out, int64_t cap_faces, void* stream);
+
 /* ---- kernel timing (bench.py roofline) ---------------------------------------------------
  * When enabled, the tensor-core path brackets its two kernels (the fused PE+MLP chain kernel and
  * the weight-gradient kernel) with CUDA events on the launching stream.  isdfb_profile_read
@@ -280,6 +323,13 @@ int isdfb_profile_read(isdfb_ctx* ctx, double* chain_ms, double* dw_ms, int64_t*
  * path (-2), buffer too small (-4).  The sweeps are SURVEY.md 8a's S1..S4 (fc_map.py:94-111, 12-22; trainer.py:981). */
 int isdfb_debug_program(int32_t n_freqs, int32_t hidden, int32_t block, int32_t mode, int32_t* steps_out,
                         int32_t max_steps);
+
+/* Host-only: the marching-cubes case table isdfb_mesh_emit uses (no CUDA call).  rows [256][32]: byte 0 = triangle count
+ * of the case (bit c of the case = corner c inside; corner bit 0 +x, 1 +y, 2 +z), then 3 edge ids per triangle (edge e:
+ * axis e >> 2, the other two axes' corner bits in (e & 3), the lower axis in bit 0); unused bytes 0xFF.  max_tris = the
+ * largest triangle count of any case.  Either pointer may be NULL, not both.  Derived from the face rule (the inside
+ * corners of an ambiguous face are separated) when first asked for.                                                  */
+int isdfb_debug_mc_table(uint8_t* rows, int32_t* max_tris);
 
 /* ---- debug hook (tests only): raw per-tile side state of the tensor-core path -------------
  * aux: fp32 arrays [n_aux][tiles_cap][256*128] in the aux layout, dwl_hi/lo: bf16 arrays

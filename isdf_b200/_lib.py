@@ -70,9 +70,15 @@ SIGNATURES = {
     "isdfb_adamw_graph": (C.c_int, [P, P, P, P, F, F, F, F, F, F, P]),
     "isdfb_adamw_set_step": (C.c_int, [P, I64, P]),
     "isdfb_grad_buffer": (C.c_int, [P, C.POINTER(P), C.POINTER(I64)]),
+    "isdfb_mesh_count": (C.c_int, [P, P, I32, C.POINTER(I64), C.POINTER(I64), P]),
+    "isdfb_mesh_emit": (C.c_int, [P, P, I32, C.POINTER(F), C.POINTER(F), P, I64, P, I64, P]),
+    "isdfb_mesh_cloud": (C.c_int, [P, P, P, I32, I32, I32, I32, I32, F, F, F, F, P, P, P]),
+    "isdfb_mesh_crop_count": (C.c_int, [P, P, I64, F, P, I64, P, I64, C.POINTER(I64), C.POINTER(I64), P]),
+    "isdfb_mesh_crop_emit": (C.c_int, [P, P, I64, P, I64, P, I64, P, I64, P]),
     "isdfb_profile_enable": (C.c_int, [P, I32]),
     "isdfb_profile_read": (C.c_int, [P, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(I64), C.POINTER(I64)]),
     "isdfb_debug_program": (C.c_int, [I32, I32, I32, I32, C.POINTER(I32), I32]),
+    "isdfb_debug_mc_table": (C.c_int, [C.POINTER(C.c_uint8), C.POINTER(I32)]),
     "isdfb_debug_buffers": (C.c_int, [P, C.POINTER(P), C.POINTER(I64), C.POINTER(P), C.POINTER(P), C.POINTER(I64),
                                       C.POINTER(I32), C.POINTER(I32), C.POINTER(I64), C.POINTER(P)]),
 }

@@ -143,6 +143,7 @@ int isdfb_destroy(isdfb_ctx* ctx) {
   if (ctx->adam_dev) cudaFree(ctx->adam_dev);
   if (ctx->grid_x) cudaFree(ctx->grid_x);
   if (ctx->sample_dev) cudaFree(ctx->sample_dev);
+  mesh_destroy(ctx);
   delete ctx;
   return ISDFB_OK;
 }
@@ -410,6 +411,51 @@ int isdfb_adamw_graph(isdfb_ctx* ctx, float* params_flat, float* m, float* v, fl
 int isdfb_adamw_set_step(isdfb_ctx* ctx, int64_t step, void* stream) {
   ENTER(ctx);
   return optim_set_step(ctx, step, st);
+}
+
+int isdfb_mesh_count(isdfb_ctx* ctx, const float* sdf, int32_t dim, int64_t* n_verts, int64_t* n_faces, void* stream) {
+  ENTER(ctx);
+  if (!sdf || !n_verts || !n_faces) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_mesh_count: null argument");
+  return mesh_count(ctx, sdf, dim, n_verts, n_faces, st);
+}
+
+int isdfb_mesh_emit(isdfb_ctx* ctx, const float* sdf, int32_t dim, const float* scale, const float* transform,
+                    float* verts, int64_t cap_verts, int32_t* faces, int64_t cap_faces, void* stream) {
+  ENTER(ctx);
+  if (!sdf) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_mesh_emit: null argument");
+  return mesh_emit(ctx, sdf, dim, scale, transform, verts, cap_verts, faces, cap_faces, st);
+}
+
+int isdfb_mesh_cloud(isdfb_ctx* ctx, const float* depth, const float* T_WC, int32_t n_frames, int32_t H, int32_t W,
+                     int32_t H_vis, int32_t W_vis, float fx, float fy, float cx, float cy, float* cloud, float* box,
+                     void* stream) {
+  ENTER(ctx);
+  if (!box || (n_frames > 0 && (!depth || !T_WC || !cloud))) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_mesh_cloud: null argument");
+  if (n_frames < 0 || H < 1 || W < 1 || H_vis < 1 || W_vis < 1)
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_mesh_cloud: bad shape (frames %d, %dx%d -> %dx%d)", n_frames, H, W, H_vis, W_vis);
+  return mesh_cloud(ctx, depth, T_WC, n_frames, H, W, H_vis, W_vis, fx, fy, cx, cy, cloud, box, st);
+}
+
+int isdfb_mesh_crop_count(isdfb_ctx* ctx, const float* cloud, int64_t n_cloud, float crop_dist, const float* verts,
+                          int64_t n_verts, const int32_t* faces, int64_t n_faces, int64_t* n_verts_kept,
+                          int64_t* n_faces_kept, void* stream) {
+  ENTER(ctx);
+  if (!n_verts_kept || !n_faces_kept || (n_cloud > 0 && !cloud) || (n_verts > 0 && !verts) || (n_faces > 0 && !faces))
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_mesh_crop_count: null argument");
+  if (n_cloud < 0 || n_verts < 0 || n_faces < 0) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_mesh_crop_count: negative size");
+  return mesh_crop_count(ctx, cloud, n_cloud, crop_dist, verts, n_verts, faces, n_faces, n_verts_kept, n_faces_kept, st);
+}
+
+int isdfb_mesh_crop_emit(isdfb_ctx* ctx, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces,
+                         float* verts_out, int64_t cap_verts, int32_t* faces_out, int64_t cap_faces, void* stream) {
+  ENTER(ctx);
+  return mesh_crop_emit(ctx, verts, n_verts, faces, n_faces, verts_out, cap_verts, faces_out, cap_faces, st);
+}
+
+int isdfb_debug_mc_table(uint8_t* rows, int32_t* max_tris) {
+  NvtxScope _nvtx(__func__);
+  if (!rows && !max_tris) return ISDFB_ERR_ARG;
+  return mesh_table_host(rows, max_tris);
 }
 
 int isdfb_grad_buffer(isdfb_ctx* ctx, float** ptr, int64_t* n_floats) {

@@ -68,6 +68,7 @@ struct isdfb_ctx {
   void* adam_dev;          // device AdamDev {step_size, bc2_sqrt, step} for the graph-safe K6
   float* grid_x;           // fp32 path: lattice points of one chunk (isdfb_mlp_forward_grid), allocated on first use
   void* sample_dev;        // device FusedSampleState {step, valid, blocks_done} of the fused fast-mode sampler
+  void* mesh;              // mesh extraction workspace (mesh.cu), created by the first isdfb_mesh_* call, grows on demand
 };
 
 extern char g_isdfb_create_err[512];
@@ -109,3 +110,14 @@ int optim_adamw_dev(isdfb_ctx* ctx, float* params_flat, float* m, float* v, floa
                     float eps, float wd, float grad_scale, cudaStream_t st);
 int optim_set_step(isdfb_ctx* ctx, int64_t step, cudaStream_t st);
 int optim_export_grads(isdfb_ctx* ctx, float* grads_flat, cudaStream_t st);
+int mesh_table_host(uint8_t* rows, int32_t* max_tris);
+void mesh_destroy(isdfb_ctx* ctx);
+int mesh_count(isdfb_ctx* ctx, const float* sdf, int dim, int64_t* n_verts, int64_t* n_faces, cudaStream_t st);
+int mesh_emit(isdfb_ctx* ctx, const float* sdf, int dim, const float* scale, const float* transform, float* verts,
+              int64_t cap_v, int32_t* faces, int64_t cap_f, cudaStream_t st);
+int mesh_cloud(isdfb_ctx* ctx, const float* depth, const float* T_WC, int n_frames, int H, int W, int Hv, int Wv,
+               float fx, float fy, float cx, float cy, float* cloud, float* box, cudaStream_t st);
+int mesh_crop_count(isdfb_ctx* ctx, const float* cloud, int64_t n_cloud, float crop_dist, const float* verts,
+                    int64_t nv, const int32_t* faces, int64_t nf, int64_t* kv, int64_t* kf, cudaStream_t st);
+int mesh_crop_emit(isdfb_ctx* ctx, const float* verts, int64_t nv, const int32_t* faces, int64_t nf, float* verts_out,
+                   int64_t cap_v, int32_t* faces_out, int64_t cap_f, cudaStream_t st);

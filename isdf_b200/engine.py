@@ -218,6 +218,73 @@ class Engine:
         self._ck(self.lib.isdfb_mlp_forward_grid(self._ctx, _ptr(lin), int(dim), sc, tr, _ptr(sdf), self._stream()))
         return sdf
 
+    # ---- N4: mesh extraction ------------------------------------------
+    def mesh_count(self, sdf):
+        """Marching-cubes counts of the lattice sdf [dim,dim,dim] (synchronous): (vertices, faces)."""
+        sdf = _f32(sdf, "sdf", self.device)
+        dim = sdf.shape[0] if sdf.dim() == 3 else -1
+        if sdf.shape != (dim, dim, dim):
+            raise ValueError("sdf must be a [dim,dim,dim] lattice, got %s" % (tuple(sdf.shape),))
+        nv, nf = C.c_int64(), C.c_int64()
+        self._ck(self.lib.isdfb_mesh_count(self._ctx, _ptr(sdf), int(dim), C.byref(nv), C.byref(nf), self._stream()))
+        return nv.value, nf.value
+
+    def mesh_emit(self, sdf, verts, faces, scale=None, transform=None):
+        """Fill verts [V,3] f32 and faces [F,3] int32 with the mesh of the lattice last passed to mesh_count; the
+        capacities are the tensors' row counts."""
+        sdf = _f32(sdf, "sdf", self.device)
+        for t, nm, dt in ((verts, "verts", torch.float32), (faces, "faces", torch.int32)):
+            if t.dtype != dt or t.device != self.device or not t.is_contiguous() or t.dim() != 2 or t.shape[1] != 3:
+                raise TypeError("%s must be a contiguous %s [N,3] tensor on %s" % (nm, dt, self.device))
+        sc = (C.c_float * 3)(*[float(v) for v in torch.as_tensor(scale).reshape(-1).tolist()]) if scale is not None else None
+        tr = None
+        if transform is not None:
+            tr = (C.c_float * 12)(*torch.as_tensor(transform, dtype=torch.float32).cpu()[:3, :4].reshape(-1).tolist())
+        self._ck(self.lib.isdfb_mesh_emit(self._ctx, _ptr(sdf), int(sdf.shape[0]), sc, tr, _ptr(verts), verts.shape[0],
+                                          _ptr(faces), faces.shape[0], self._stream()))
+        return verts, faces
+
+    def mesh(self, sdf, scale=None, transform=None):
+        """Marching cubes at level 0 (draw3D.draw_mesh): vertices [V,3] f32 in the world, faces [F,3] int32."""
+        nv, nf = self.mesh_count(sdf)
+        verts = torch.empty(nv, 3, dtype=torch.float32, device=self.device)
+        faces = torch.empty(nf, 3, dtype=torch.int32, device=self.device)
+        return self.mesh_emit(sdf, verts, faces, scale=scale, transform=transform)
+
+    def mesh_cloud(self, depth, T_WC, H_vis, W_vis, fx, fy, cx, cy):
+        """Keyframe point cloud of mesh_rec: depth [F,H,W] nearest-resized to (H_vis, W_vis), back-projected with the
+        reduced intrinsics, moved to the world.  Returns (cloud [F*H_vis*W_vis, 3], box [6] = min xyz, max xyz)."""
+        depth, T_WC = _f32(depth, "depth", self.device), _f32(T_WC, "T_WC", self.device)
+        F_, H, W = depth.shape
+        if T_WC.shape != (F_, 4, 4):
+            raise ValueError("T_WC must be [%d,4,4]" % F_)
+        cloud = torch.empty(F_ * int(H_vis) * int(W_vis), 3, dtype=torch.float32, device=self.device)
+        box = torch.empty(6, dtype=torch.float32, device=self.device)
+        self._ck(self.lib.isdfb_mesh_cloud(self._ctx, _ptr(depth), _ptr(T_WC), F_, H, W, int(H_vis), int(W_vis),
+                                           float(fx), float(fy), float(cx), float(cy), _ptr(cloud), _ptr(box),
+                                           self._stream()))
+        return cloud, box
+
+    def mesh_crop(self, cloud, verts, faces, crop_dist):
+        """Keep the faces with a vertex closer than crop_dist to the cloud, then the vertices they use (renumbered in
+        order).  Returns (vertices [V',3] f32, faces [F',3] int32)."""
+        cloud, verts = _f32(cloud, "cloud", self.device), _f32(verts, "verts", self.device)
+        if faces.dtype != torch.int32 or faces.device != self.device:
+            raise TypeError("faces must be int32 on %s" % self.device)
+        faces = faces.contiguous()
+        for t, nm in ((cloud, "cloud"), (verts, "verts"), (faces, "faces")):
+            if t.dim() != 2 or t.shape[1] != 3:
+                raise ValueError("%s must be [N,3], got %s" % (nm, tuple(t.shape)))
+        nv, nf = verts.shape[0], faces.shape[0]
+        kv, kf = C.c_int64(), C.c_int64()
+        self._ck(self.lib.isdfb_mesh_crop_count(self._ctx, _ptr(cloud), cloud.shape[0], float(crop_dist), _ptr(verts), nv,
+                                                _ptr(faces), nf, C.byref(kv), C.byref(kf), self._stream()))
+        v_out = torch.empty(kv.value, 3, dtype=torch.float32, device=self.device)
+        f_out = torch.empty(kf.value, 3, dtype=torch.int32, device=self.device)
+        self._ck(self.lib.isdfb_mesh_crop_emit(self._ctx, _ptr(verts), nv, _ptr(faces), nf, _ptr(v_out), kv.value,
+                                               _ptr(f_out), kf.value, self._stream()))
+        return v_out, f_out
+
     # ---- N2 ----------------------------------------------------------
     def bounds_pc(self, pc, z_vals, depth_sample, ray_valid=None):
         """loss.bounds_pc (loss.py:56-89): bounds [R,S] and target directions [R,S,3] (row 0 unused)."""

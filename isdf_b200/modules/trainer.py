@@ -14,7 +14,8 @@ sample_points / sdf_eval_and_loss.  One step launches (reference trainer.py:951-
 Two RNG modes: "reference" consumes torch / numpy generators in exactly the reference's order
 (SURVEY.md appendix B; one host sync for the data-dependent ray compaction, as in the reference);
 "fast" keeps fixed shapes with a validity mask and never synchronises inside the step.
-Visualisation, evaluation and mesh extraction are out of scope (SURVEY.md section 2) and raise.
+Visualisation and evaluation are out of scope (SURVEY.md section 2) and raise; mesh extraction (mesh_rec, write_mesh)
+runs on the device (isdfb_mesh_*).
 """
 import copy
 import json
@@ -28,15 +29,24 @@ from ..datasets import dataset as ds
 from ..datasets.data_util import FrameData
 from ..engine import make_camera, make_loss_cfg
 from ..eval.metrics import start_timing, end_timing
+from ..geometry import mesh as mesh_io
 from ..geometry import transform
 from .. import parallel
 from . import embedding, fc_map, render, sample
 
 _OUT_OF_SCOPE = ("view_sdf", "latest_frame_vis", "update_vis_vars", "frames_vis", "draw_3D", "draw_obj_3D",
-                 "obj_slices_vis", "write_slices", "write_mesh", "mesh_rec", "eval_fixed", "eval_sdf",
+                 "obj_slices_vis", "write_slices", "eval_fixed", "eval_sdf",
                  "eval_object_sdf", "eval_mesh", "compute_slices", "keyframe_vis", "slices_vis", "render_depth_vis",
                  "render_normals_vis", "to_topdown", "load_gt_sdf", "check_gt_sdf", "eval_sdf_visible", "eval_sdf_volume",
                  "eval_traj_cost")
+
+
+def _axis_aligned_box(lo, hi):
+    """The box of a point set with corners lo, hi: (T_extent_to_scene, bounds_extents, scene_center)."""
+    lo, hi = np.asarray(lo, dtype=np.float64), np.asarray(hi, dtype=np.float64)
+    T_extent_to_scene = np.eye(4)
+    T_extent_to_scene[:3, 3] = -(lo + hi) / 2
+    return T_extent_to_scene, hi - lo, (lo + hi) / 2
 
 
 class FusedAdamW:
@@ -853,28 +863,34 @@ class Trainer:
         trimesh.bounds.oriented_bounds), or an [N,3] point array / an object with `.vertices`, for
         which the AXIS-ALIGNED box is used."""
         if "realsense_franka" in self.dataset_format and T_extent_to_scene is None:
-            ws = self.config["workspace"]
-            a = np.deg2rad(ws["rotate_z"])
-            T_extent_to_scene = np.eye(4)
-            T_extent_to_scene[:2, :2] = [[np.cos(a), -np.sin(a)], [np.sin(a), np.cos(a)]]
-            T_extent_to_scene[:3, 3] = np.array(ws["offset"])
-            bounds_extents, scene_center = np.array(ws["extents"]), np.array(ws["center"])
+            T_extent_to_scene, bounds_extents, scene_center = self._workspace_box()
         if T_extent_to_scene is None:
             if scene_mesh is None:
                 raise ValueError("set_scene_properties needs an oriented box or a point set")
             pts = np.asarray(getattr(scene_mesh, "vertices", scene_mesh), dtype=np.float64).reshape(-1, 3)
-            lo, hi = pts.min(axis=0), pts.max(axis=0)
-            T_extent_to_scene = np.eye(4)
-            T_extent_to_scene[:3, 3] = -(lo + hi) / 2
-            bounds_extents = hi - lo
-            scene_center = (lo + hi) / 2
+            T_extent_to_scene, bounds_extents, scene_center = _axis_aligned_box(pts.min(axis=0), pts.max(axis=0))
         T_extent_to_scene = np.asarray(T_extent_to_scene, dtype=np.float64)
         bounds_extents = np.asarray(bounds_extents, dtype=np.float64)
-        self.scene_center = scene_center
         self.inv_bounds_transform = torch.from_numpy(T_extent_to_scene).float().to(self.device)
         if getattr(self, "sdf_map", None) is not None:
             # called after load_networks: the encoding's transform follows (SDFMap.engine() re-creates its context)
             self.sdf_map.positional_encoding.transform = self.inv_bounds_transform
+        self._set_lattice(T_extent_to_scene, bounds_extents, scene_center)
+
+    def _workspace_box(self):
+        """The franka formats' own scene box from the config's workspace entry (trainer.py:113-119):
+        (T_extent_to_scene, bounds_extents, scene_center)."""
+        ws = self.config["workspace"]
+        a = np.deg2rad(ws["rotate_z"])
+        T_extent_to_scene = np.eye(4)
+        T_extent_to_scene[:2, :2] = [[np.cos(a), -np.sin(a)], [np.sin(a), np.cos(a)]]
+        T_extent_to_scene[:3, 3] = np.array(ws["offset"])
+        return T_extent_to_scene, np.array(ws["extents"]), np.array(ws["center"])
+
+    def _set_lattice(self, T_extent_to_scene, bounds_extents, scene_center):
+        """The query-lattice half of set_scene_properties (trainer.py:124-156): box transform, grid scale, the
+        grid_dim^3 lattice generator, the up axis and the crop distance.  The positional encoding is not touched."""
+        self.scene_center = scene_center
         self.bounds_transform_np = np.linalg.inv(T_extent_to_scene)
         self.bounds_transform = torch.from_numpy(self.bounds_transform_np).float().to(self.device)
         grid_range = [-1.0, 1.0]
@@ -892,6 +908,51 @@ class Trainer:
         self.grid_up = self.bounds_transform_np[:3, self.up_ix]
         self.up_aligned = np.dot(self.grid_up, self.up) > 0
         self.crop_dist = 0.1 if "franka" in self.dataset_format else 0.25
+
+    # ---- mesh extraction (trainer.py:1500-1556) ------------------------------------------------
+    def mesh_rec(self, crop_mesh_with_pc=True):
+        """Marching cubes over get_sdf_grid, cropped to the keyframes' point cloud (trainer.py:1500-1542), all on the
+        device.  Without a ground-truth scene, incremental runs first re-derive the lattice box as set_scene_properties
+        does: from that cloud (axis-aligned: the reference's trimesh oriented box is not available), or, for the franka
+        formats, from the config's workspace.  The positional encoding keeps its transform, so meshing never changes
+        the model.  Returns a Mesh (vertices float64 [V,3], faces int64 [F,3])."""
+        eng = self.sdf_map.engine()
+        f = self.frames
+        if len(f) == 0:
+            raise RuntimeError("mesh_rec needs at least one keyframe")
+        cloud, box = eng.mesh_cloud(f.depth_batch, f.T_WC_batch, self.H_vis, self.W_vis, self.fx_vis, self.fy_vis,
+                                    self.cx_vis, self.cy_vis)
+        if self.gt_scene is False and self.incremental:
+            # the reference calls set_scene_properties(cloud) here (trainer.py:1514-1516), which takes the franka
+            # formats' workspace box from the config and ignores the cloud (trainer.py:113-119)
+            if "realsense_franka" in self.dataset_format:
+                scene_box = self._workspace_box()
+            else:
+                lo_hi = box.double().cpu().numpy()
+                if not np.isfinite(lo_hi).all():
+                    raise RuntimeError("mesh_rec: the keyframes hold no finite depth to derive the scene box from")
+                scene_box = _axis_aligned_box(lo_hi[:3], lo_hi[3:])
+            self._set_lattice(*scene_box)
+        sdf = self.get_sdf_grid()
+        verts, faces = eng.mesh(sdf.contiguous(), scale=self.scene_scale, transform=self.bounds_transform)
+        if crop_mesh_with_pc:
+            verts, faces = eng.mesh_crop(cloud, verts, faces, self.crop_dist)
+        if self.new_grid_dim is not None:
+            self.grid_dim = self.new_grid_dim
+            self.grid_pc = getattr(self, "new_grid_pc", None)
+            self.new_grid_dim = None
+            self.new_grid_pc = None
+        return mesh_io.Mesh(verts.cpu().numpy(), faces.cpu().numpy())
+
+    def write_mesh(self, filename, im_pose=None):
+        """mesh_rec() as a binary PLY (trainer.py:1544-1556).  Rendering the mesh to an image at im_pose needs an
+        off-screen renderer, which is not part of this package."""
+        if im_pose is not None:
+            raise NotImplementedError("write_mesh(im_pose=...) renders the mesh off-screen (trimesh / pyglet); only the "
+                                      "PLY file is written here")
+        data = mesh_io.export_ply(self.mesh_rec())
+        with open(filename, "wb") as out:
+            out.write(data)
 
     def get_sdf_grid(self):
         """SDF on the grid_dim^3 lattice (trainer.py:1426-1444): one K2 call, chunked inside the library
