@@ -35,7 +35,7 @@ def run_train(engine, sd, batch, noise, cfg, device):
     """One K4 call; returns dict(sdf, g, loss_mat, sums, grads(list in state-dict order))."""
     engine.pack_weights(flat_params(sd, device))
     engine.zero_grad()
-    b = {k: v.to(device=device, dtype=torch.float32) for k, v in batch.items()}
+    b = {k: (v.to(device=device, dtype=torch.float32) if v is not None else None) for k, v in batch.items()}
     R, S = b["z_vals"].shape
     pcb = pcv = None
     if cfg.get("bounds_method", "ray") == "pc":          # N2: bounds from the all-pairs kernel
@@ -65,7 +65,7 @@ def oracle_train(sd, batch, noise, cfg, dtype=torch.float64):
     cfg = dict(cfg)
     if cfg.get("transform") is not None:
         cfg["transform"] = cfg["transform"].to(dtype)
-    b = {k: v.to(dtype) for k, v in batch.items()}
+    b = {k: (v.to(dtype) if v is not None else None) for k, v in batch.items()}
     nz = noise.to(dtype) if (noise is not None and cfg["noise_std"]) else None
     return O.step_sweeps(layers, b, cfg, nz)
 
