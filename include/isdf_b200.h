@@ -307,6 +307,37 @@ int isdfb_mesh_crop_count(isdfb_ctx* ctx, const float* cloud, int64_t n_cloud, f
 int isdfb_mesh_crop_emit(isdfb_ctx* ctx, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces,
                          float* verts_out, int64_t cap_verts, int32_t* faces_out, int64_t cap_faces, void* stream);
 
+/* ---- evaluation against a ground-truth SDF (Trainer.load_gt_sdf / eval_sdf / eval_object_sdf) -------------------
+ * isdfb_gt_sdf_sample: sdf_util.sdf_interpolator + eval_sdf_interp (sdf_util.py:151-216, trainer.py:446-453), i.e.
+ *   scipy RegularGridInterpolator(method "linear") over the axes np.arange(d) * spacing + origin (get_grid_pts, the
+ *   transform.txt diagonal and translation).  lattice: fp32 [nx,ny,nz] (device, C order); origin / spacing [3] (host);
+ *   exactly one of pts_f32 / pts_f64 [n,3] (device).  out [n] fp64, in_bounds [n] bytes.  Index and fraction
+ *   arithmetic in fp64 with node coordinates i * spacing + origin; the cell grid[i] <= x < grid[i+1] with the last plane
+ *   in the last cell; bounds inclusive.  A point outside the box gets `fill` and byte 0; a point with a NaN coordinate
+ *   gets NaN and byte 1 (scipy writes NaN over the fill), so the byte is eval_sdf_interp's handle_oob='mask' mask.
+ *   Every axis needs >= 2 nodes and spacing > 0.                                                                     */
+int isdfb_gt_sdf_sample(isdfb_ctx* ctx, const float* lattice, int32_t nx, int32_t ny, int32_t nz,
+                        const double* origin /*[3], host*/, const double* spacing /*[3], host*/, const float* pts_f32,
+                        const double* pts_f64, int64_t n, double fill, double* out, uint8_t* in_bounds, void* stream);
+
+/* isdfb_sdf_error_stats: the reduction of eval_sdf (trainer.py:1831-1864, metrics.binned_losses metrics.py:133-158,
+ *   metrics.chomp_cost metrics.py:95-104).  A point counts iff in_bounds, valid (NULL: all valid; fast-mode rays are
+ *   masked, not compacted) and gt != 0 (the GT lattice is 0 inside walls).  out [17] fp64 (device): [0] count,
+ *   [1] sum |pred - gt|, [2..7] counts and [8..13] sums of |pred - gt| in the open bins (-1e99, 0, 0.1, 0.2, 0.5, 1,
+ *   1e99) of gt, [14..16] sums of |chomp(pred) - chomp(gt)| for epsilon 1, 1.5, 2, chomp(pred) in fp32 and chomp(gt)
+ *   in fp64.  Per-block partials over a grid fixed by n and a fixed-order final sum: two calls agree bitwise.       */
+#define ISDFB_EVAL_NSTATS 17
+int isdfb_sdf_error_stats(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* in_bounds,
+                          const uint8_t* valid, int64_t n, double* out, void* stream);
+
+/* isdfb_points_visible: geometry.frustum.is_visible_torch (frustum.py:87-135) reduced over the frames as
+ *   trainer.py:1976-1983 does.  pts [n,3], T_CW [n_frames,4,4] (the inverse of T_WC, fp32), depth [n_frames,H,W], all
+ *   fp32 on the device.  vis[p] = 1 iff some frame has 0 < u < W, 0 < v < H for the fp32 projection of p, and
+ *   0 < z < depth[(int)v, (int)u] + trunc.                                                                             */
+int isdfb_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float* T_CW, const float* depth,
+                         int32_t n_frames, int32_t H, int32_t W, float fx, float fy, float cx, float cy, float trunc,
+                         uint8_t* vis, void* stream);
+
 /* ---- kernel timing (bench.py roofline) ---------------------------------------------------
  * When enabled, the tensor-core path brackets its two kernels (the fused PE+MLP chain kernel and
  * the weight-gradient kernel) with CUDA events on the launching stream.  isdfb_profile_read

@@ -144,6 +144,7 @@ int isdfb_destroy(isdfb_ctx* ctx) {
   if (ctx->grid_x) cudaFree(ctx->grid_x);
   if (ctx->sample_dev) cudaFree(ctx->sample_dev);
   mesh_destroy(ctx);
+  eval_destroy(ctx);
   delete ctx;
   return ISDFB_OK;
 }
@@ -450,6 +451,39 @@ int isdfb_mesh_crop_emit(isdfb_ctx* ctx, const float* verts, int64_t n_verts, co
                          float* verts_out, int64_t cap_verts, int32_t* faces_out, int64_t cap_faces, void* stream) {
   ENTER(ctx);
   return mesh_crop_emit(ctx, verts, n_verts, faces, n_faces, verts_out, cap_verts, faces_out, cap_faces, st);
+}
+
+int isdfb_gt_sdf_sample(isdfb_ctx* ctx, const float* lattice, int32_t nx, int32_t ny, int32_t nz, const double* origin,
+                        const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double fill,
+                        double* out, uint8_t* in_bounds, void* stream) {
+  ENTER(ctx);
+  if (!origin || !spacing || n < 0 || (n > 0 && (!lattice || !out || !in_bounds || (!pts_f32 == !pts_f64))))
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_sample: null argument (or both / neither point arrays)");
+  if (nx < 2 || ny < 2 || nz < 2)
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_sample: lattice %dx%dx%d needs >= 2 nodes per axis", nx, ny, nz);
+  for (int d = 0; d < 3; ++d)
+    if (!(spacing[d] > 0.0) || !isfinite(origin[d]) || !isfinite(spacing[d]))
+      ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_sample: axis %d origin %g spacing %g", d, origin[d], spacing[d]);
+  return eval_gt_sample(ctx, lattice, nx, ny, nz, origin, spacing, pts_f32, pts_f64, n, fill, out, in_bounds, st);
+}
+
+int isdfb_sdf_error_stats(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* in_bounds,
+                          const uint8_t* valid, int64_t n, double* out, void* stream) {
+  ENTER(ctx);
+  if (!out || n < 0 || (n > 0 && (!pred || !gt || !in_bounds)))
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_sdf_error_stats: null argument");
+  return eval_error_stats(ctx, pred, gt, in_bounds, valid, n, out, st);
+}
+
+int isdfb_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float* T_CW, const float* depth,
+                         int32_t n_frames, int32_t H, int32_t W, float fx, float fy, float cx, float cy, float trunc,
+                         uint8_t* vis, void* stream) {
+  ENTER(ctx);
+  if (n < 0 || n_frames < 0 || H < 1 || W < 1)
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_points_visible: bad shape (n %lld, frames %d, %dx%d)", (long long)n, n_frames, H, W);
+  if (n > 0 && (!pts || !vis || (n_frames > 0 && (!T_CW || !depth))))
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_points_visible: null argument");
+  return eval_points_visible(ctx, pts, n, T_CW, depth, n_frames, H, W, fx, fy, cx, cy, trunc, vis, st);
 }
 
 int isdfb_debug_mc_table(uint8_t* rows, int32_t* max_tris) {

@@ -69,6 +69,7 @@ struct isdfb_ctx {
   float* grid_x;           // fp32 path: lattice points of one chunk (isdfb_mlp_forward_grid), allocated on first use
   void* sample_dev;        // device FusedSampleState {step, valid, blocks_done} of the fused fast-mode sampler
   void* mesh;              // mesh extraction workspace (mesh.cu), created by the first isdfb_mesh_* call, grows on demand
+  void* eval;              // per-block partial sums of isdfb_sdf_error_stats (eval.cu), allocated on first use
 };
 
 extern char g_isdfb_create_err[512];
@@ -121,3 +122,12 @@ int mesh_crop_count(isdfb_ctx* ctx, const float* cloud, int64_t n_cloud, float c
                     int64_t nv, const int32_t* faces, int64_t nf, int64_t* kv, int64_t* kf, cudaStream_t st);
 int mesh_crop_emit(isdfb_ctx* ctx, const float* verts, int64_t nv, const int32_t* faces, int64_t nf, float* verts_out,
                    int64_t cap_v, int32_t* faces_out, int64_t cap_f, cudaStream_t st);
+void eval_destroy(isdfb_ctx* ctx);
+int eval_gt_sample(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz, const double* origin,
+                   const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double fill,
+                   double* out, uint8_t* inb, cudaStream_t st);
+int eval_error_stats(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, const uint8_t* valid,
+                     int64_t n, double* out, cudaStream_t st);
+int eval_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float* T_CW, const float* depth,
+                        int n_frames, int H, int W, float fx, float fy, float cx, float cy, float trunc, uint8_t* vis,
+                        cudaStream_t st);

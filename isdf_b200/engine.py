@@ -285,6 +285,60 @@ class Engine:
                                                _ptr(f_out), kf.value, self._stream()))
         return v_out, f_out
 
+    # ---- evaluation against a ground-truth SDF -------------------------
+    def gt_sdf_sample(self, lattice, origin, spacing, pts, fill=0.0):
+        """Trilinear interpolation of the fp32 lattice [nx,ny,nz] with nodes i * spacing + origin at pts [...,3]
+        (float32 or float64), as scipy's RegularGridInterpolator over sdf_util.get_grid_pts.  Returns (values fp64 [...],
+        in-bounds uint8 [...]); out-of-bounds points get `fill`, a NaN coordinate gives NaN and byte 1."""
+        lattice = _f32(lattice, "lattice", self.device)
+        if lattice.dim() != 3:
+            raise ValueError("lattice must be [nx,ny,nz], got %s" % (tuple(lattice.shape),))
+        if pts.device != self.device or pts.dtype not in (torch.float32, torch.float64) or pts.shape[-1] != 3:
+            raise TypeError("pts must be a float32 or float64 [...,3] tensor on %s" % self.device)
+        pts = pts.contiguous()
+        shape = pts.shape[:-1]
+        out = torch.empty(shape, dtype=torch.float64, device=self.device)
+        inb = torch.empty(shape, dtype=torch.uint8, device=self.device)
+        o = (C.c_double * 3)(*[float(v) for v in origin])
+        s = (C.c_double * 3)(*[float(v) for v in spacing])
+        f64 = pts.dtype == torch.float64
+        self._ck(self.lib.isdfb_gt_sdf_sample(self._ctx, _ptr(lattice), *[int(d) for d in lattice.shape], o, s,
+                                              _ptr(None if f64 else pts), _ptr(pts if f64 else None), pts.numel() // 3,
+                                              float(fill), _ptr(out), _ptr(inb), self._stream()))
+        return out, inb
+
+    def sdf_error_stats(self, pred, gt, in_bounds, valid=None):
+        """The 17 fp64 sums of eval_sdf (device tensor): count, sum |pred - gt|, six bin counts, six bin sums, three
+        CHOMP-difference sums, over the points in bounds, valid and with gt != 0."""
+        pred = _f32(pred, "pred", self.device).reshape(-1)
+        n = pred.numel()
+        if gt.dtype != torch.float64 or gt.device != self.device or gt.numel() != n:
+            raise TypeError("gt must be float64 on %s with one value per prediction" % self.device)
+        masks = []
+        for t, nm in ((in_bounds, "in_bounds"), (valid, "valid")):
+            if t is not None and (t.device != self.device or t.numel() != n):
+                raise ValueError("%s must have one byte per prediction on %s" % (nm, self.device))
+            masks.append(None if t is None else t.reshape(-1).to(torch.uint8).contiguous())
+        out = torch.empty(17, dtype=torch.float64, device=self.device)
+        self._ck(self.lib.isdfb_sdf_error_stats(self._ctx, _ptr(pred), _ptr(gt.reshape(-1).contiguous()),
+                                                _ptr(masks[0]), _ptr(masks[1]), n, _ptr(out), self._stream()))
+        return out
+
+    def points_visible(self, pts, T_CW, depth, fx, fy, cx, cy, trunc):
+        """uint8 [N]: 1 iff some frame of depth [F,H,W] (camera-from-world T_CW [F,4,4]) sees the point within trunc
+        behind its surface (frustum.is_visible_torch, any over the frames)."""
+        pts, T_CW, depth = _f32(pts, "pts", self.device), _f32(T_CW, "T_CW", self.device), _f32(depth, "depth", self.device)
+        if pts.dim() != 2 or pts.shape[1] != 3:
+            raise ValueError("pts must be [N,3], got %s" % (tuple(pts.shape),))
+        F_, H, W = depth.shape
+        if T_CW.shape != (F_, 4, 4):
+            raise ValueError("T_CW must be [%d,4,4]" % F_)
+        vis = torch.empty(pts.shape[0], dtype=torch.uint8, device=self.device)
+        self._ck(self.lib.isdfb_points_visible(self._ctx, _ptr(pts), pts.shape[0], _ptr(T_CW), _ptr(depth), F_, H, W,
+                                               float(fx), float(fy), float(cx), float(cy), float(trunc), _ptr(vis),
+                                               self._stream()))
+        return vis
+
     # ---- N2 ----------------------------------------------------------
     def bounds_pc(self, pc, z_vals, depth_sample, ray_valid=None):
         """loss.bounds_pc (loss.py:56-89): bounds [R,S] and target directions [R,S,3] (row 0 unused)."""

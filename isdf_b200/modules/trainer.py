@@ -14,8 +14,9 @@ sample_points / sdf_eval_and_loss.  One step launches (reference trainer.py:951-
 Two RNG modes: "reference" consumes torch / numpy generators in exactly the reference's order
 (SURVEY.md appendix B; one host sync for the data-dependent ray compaction, as in the reference);
 "fast" keeps fixed shapes with a validity mask and never synchronises inside the step.
-Visualisation and evaluation are out of scope (SURVEY.md section 2) and raise; mesh extraction (mesh_rec, write_mesh)
-runs on the device (isdfb_mesh_*).
+Visualisation is out of scope (SURVEY.md section 2) and raises; mesh extraction (mesh_rec, write_mesh) runs on the
+device (isdfb_mesh_*), and so does the evaluation against a ground-truth SDF (load_gt_sdf, eval_sdf, eval_object_sdf:
+isdfb_gt_sdf_sample, isdfb_sdf_error_stats, isdfb_points_visible).
 """
 import copy
 import json
@@ -35,10 +36,49 @@ from .. import parallel
 from . import embedding, fc_map, render, sample
 
 _OUT_OF_SCOPE = ("view_sdf", "latest_frame_vis", "update_vis_vars", "frames_vis", "draw_3D", "draw_obj_3D",
-                 "obj_slices_vis", "write_slices", "eval_fixed", "eval_sdf",
-                 "eval_object_sdf", "eval_mesh", "compute_slices", "keyframe_vis", "slices_vis", "render_depth_vis",
-                 "render_normals_vis", "to_topdown", "load_gt_sdf", "check_gt_sdf", "eval_sdf_visible", "eval_sdf_volume",
-                 "eval_traj_cost")
+                 "obj_slices_vis", "write_slices", "eval_fixed", "eval_mesh", "compute_slices", "keyframe_vis",
+                 "slices_vis", "render_depth_vis", "render_normals_vis", "to_topdown", "check_gt_sdf", "eval_traj_cost")
+
+# the evaluation frames' depth transform (eval_pts.get_cache_dataset): fixed scale per format, far values zeroed at 12 m
+_EVAL_DEPTH_SCALE = {"replicaCAD": 1. / 3276.75, "ScanNet": 1. / 1000.}
+_EVAL_FRAME_STRIDE = 5
+
+
+class GtSdfInterp:
+    """A ground-truth SDF lattice resident on the device, with the parts of scipy's RegularGridInterpolator that
+    sdf_util.eval_sdf_interp and the Trainer use: `bounds_error`, `fill_value` and `__call__` on a numpy array or torch
+    tensor [..., 3], which returns a float64 numpy array [...].  Values come from isdfb_gt_sdf_sample (trilinear, fp64
+    arithmetic over the fp32 lattice).  With bounds_error set, a point outside the lattice (or with a NaN coordinate)
+    raises ValueError, as scipy does; otherwise such a point gets fill_value and a NaN coordinate gives NaN.
+    fill_value=None (scipy's extrapolation) is not provided."""
+
+    def __init__(self, engine, lattice, transform):
+        self._engine = engine                       # callable -> the Engine (a Trainer's engine may be re-created)
+        self.lattice = lattice                      # fp32 [nx,ny,nz] on the device
+        transform = np.asarray(transform, dtype=np.float64)
+        self.origin = [float(v) for v in transform[:3, 3]]
+        self.spacing = [float(transform[d, d]) for d in range(3)]
+        self.bounds_error = True
+        self.fill_value = np.nan
+
+    def sample(self, pts, fill):
+        """pts: float32 / float64 [..., 3] on the lattice's device -> (fp64 values, uint8 in-bounds) on the device."""
+        return self._engine().gt_sdf_sample(self.lattice, self.origin, self.spacing, pts, fill=fill)
+
+    def __call__(self, xi):
+        pts = xi.detach() if torch.is_tensor(xi) else torch.from_numpy(np.asarray(xi))
+        if pts.dtype not in (torch.float32, torch.float64):
+            pts = pts.double()
+        if pts.shape[-1] != 3:
+            raise ValueError("points must be [..., 3], got %s" % (tuple(pts.shape),))
+        if not self.bounds_error and self.fill_value is None:
+            raise NotImplementedError("fill_value=None (extrapolation) is not provided")
+        pts = pts.to(self.lattice.device)
+        fill = 0.0 if self.bounds_error else float(self.fill_value)
+        vals, inb = self.sample(pts, fill)
+        if self.bounds_error and pts.numel() and not bool((inb.bool().all() & ~torch.isnan(pts).any()).item()):
+            raise ValueError("One of the requested xi is out of the ground-truth SDF lattice")
+        return vals.cpu().numpy()
 
 
 def _axis_aligned_box(lo, hi):
@@ -134,6 +174,7 @@ class Trainer:
         self.optim_frames = 0
         self.gt_depth_vis = self.gt_im_vis = None
         self.gt_sdf_interp = self.stage_sdf_interp = self.sdf_dims = self.sdf_transform = None
+        self._eval_frames = None
         self.grid_dim, self.new_grid_dim, self.chunk_size = grid_dim, None, 100000
         if isinstance(config_file, dict):
             self.config = copy.deepcopy(config_file)
@@ -187,6 +228,8 @@ class Trainer:
         self._last_pts = None
         self._t_events = None
         self._lin_cache = {}
+        if self.do_eval and self.sdf_transf_file is not None:
+            self.load_gt_sdf()                         # trainer.py:93-95
 
     def __getattr__(self, name):
         if name in _OUT_OF_SCOPE:
@@ -225,12 +268,16 @@ class Trainer:
         if self.dataset_format != "realsense_franka_offline":
             self.ims_file = os.path.join(self.ims_file, "results")
         self.obj_bounds_file = None
-        self.gt_sdf_file = None
+        if os.path.exists(self.seq_dir + "/obj_bounds.txt"):
+            self.obj_bounds_file = self.seq_dir + "/obj_bounds.txt"
+        self.gt_sdf_file = self.stage_sdf_file = self.sdf_transf_file = None
         self.scene_file = None
         if "gt_sdf_dir" in d:
             self.gt_scene = True
             self.scene_file = d["gt_sdf_dir"] + "mesh.obj"
             self.gt_sdf_file = d["gt_sdf_dir"] + "/1cm/sdf.npy"
+            self.stage_sdf_file = d["gt_sdf_dir"] + "/1cm/stage_sdf.npy"
+            self.sdf_transf_file = d["gt_sdf_dir"] + "/1cm/transform.txt"
         self.scannet_dir = d.get("scannet_dir")
         self.indices = d.get("im_indices")
         self.noisy_depth = bool(d.get("noisy_depth", 0))
@@ -980,13 +1027,18 @@ class Trainer:
         self._grid_lin = None                            # an explicit point set replaces the generated lattice
 
     def get_sdf_grid_pc(self, include_gt=False, mask_near_pc=False):
-        """[dim,dim,dim,4] numpy array of (x, y, z, sdf) (trainer.py:1446-1481)."""
-        if include_gt or mask_near_pc:
-            raise NotImplementedError("GT-SDF interpolation and the KD-tree crop belong to the evaluation / "
-                                      "visualisation tool-chain (out of scope)")
+        """[dim,dim,dim,4] numpy array of (x, y, z, sdf) (trainer.py:1446-1481); with include_gt and a loaded GT SDF a
+        fifth channel holds the GT value at each lattice point (0 outside the GT lattice) and the array is float64."""
+        if mask_near_pc:
+            raise NotImplementedError("the KD-tree crop belongs to the visualisation tool-chain (out of scope)")
         sdf_grid = self.get_sdf_grid()
         grid_pc = self.grid_pc.reshape(self.grid_dim, self.grid_dim, self.grid_dim, 3)
-        return torch.cat((grid_pc, sdf_grid[..., None]), dim=-1).cpu().numpy(), None
+        sdf_grid_pc = torch.cat((grid_pc, sdf_grid[..., None]), dim=-1).cpu().numpy()
+        if include_gt and self.gt_sdf_interp is not None:
+            gt_sdf, _ = self.gt_sdf_interp.sample(self.grid_pc, fill=0.0)
+            gt_sdf = gt_sdf.reshape(self.grid_dim, self.grid_dim, self.grid_dim).cpu().numpy()
+            sdf_grid_pc = np.concatenate((sdf_grid_pc, gt_sdf[..., None]), axis=-1)
+        return sdf_grid_pc, None
 
     def sdf_fn(self, pts):
         """numpy [..,3] -> numpy sdf (trainer.py:2066-2070)."""
@@ -1021,3 +1073,151 @@ class Trainer:
             depth_vals = render.sdf_render_depth(z_up, self.sdf_map(pc_up))
         normals = render.render_normals(T_WC, depth_vals[None, ...], self.sdf_map, self.dirs_C_vis_up)
         return depth_vals.view(self.H_vis_up, self.W_vis_up), normals.view(self.H_vis_up, self.W_vis_up, 3)
+
+    # ---- evaluation against the ground-truth SDF (trainer.py:446-453, 1815-2008) ------------------------------------
+    def load_gt_sdf(self):
+        """The GT lattice <gt_sdf_dir>/1cm/sdf.npy (absolute values for ScanNet) and its transform.txt; the lattice is
+        uploaded once as fp32 behind gt_sdf_interp (a GtSdfInterp)."""
+        for f in (self.gt_sdf_file, self.sdf_transf_file):
+            if f is None or not os.path.isfile(f):
+                raise FileNotFoundError("ground-truth SDF file not found: %s" % f)
+        sdf_grid = np.load(self.gt_sdf_file)
+        if self.dataset_format == "ScanNet":
+            sdf_grid = np.abs(sdf_grid)
+        self.sdf_transform = np.loadtxt(self.sdf_transf_file)
+        self.gt_sdf_interp = self._upload_lattice(sdf_grid, self.sdf_transform)
+        self.sdf_dims = torch.tensor(sdf_grid.shape)
+
+    def _upload_lattice(self, grid, transform):
+        if grid.ndim != 3:
+            raise ValueError("a ground-truth SDF lattice must be 3-D, got shape %s" % (grid.shape,))
+        lattice = torch.from_numpy(np.ascontiguousarray(grid, dtype=np.float32)).to(self.device)
+        return GtSdfInterp(self.sdf_map.engine, lattice, transform)
+
+    def _eval_frame_data(self):
+        """The evaluation frames of eval_pts.get_cache_dataset: every 5th frame of the sequence, read with the fixed
+        depth scale of the format and a 12 m cut (no noisy depth); incremental runs see the frames before
+        int(tot_step_time * fps).  Kept on the device and extended as the run advances.  (depth [F,H,W], T_WC [F,4,4])"""
+        if self.dataset_format not in _EVAL_DEPTH_SCALE:
+            raise NotImplementedError("evaluation frames are defined for the replicaCAD and ScanNet formats only, "
+                                      "not %r" % self.dataset_format)
+        keep = np.arange(0, len(self.scene_dataset), _EVAL_FRAME_STRIDE)
+        if self.incremental:
+            keep = keep[keep < int(self.tot_step_time * self.fps)]
+        if len(keep) == 0:
+            raise RuntimeError("no evaluation frame yet: the run has not reached frame 0 (tot_step_time %g s)"
+                               % self.tot_step_time)
+        ef = self._eval_frames
+        if ef is None:
+            tf = ds.depth_scale_filter(_EVAL_DEPTH_SCALE[self.dataset_format], 12.0)
+            if self.dataset_format == "ScanNet":
+                reader = ds.ScanNetDataset(self.scannet_dir, traj_file=self.traj_file, depth_transform=tf)
+            else:
+                reader = ds.ReplicaDataset(self.ims_file, traj_file=self.traj_file, depth_transform=tf, col_ext=".png")
+            ef = self._eval_frames = {"reader": reader, "n": 0, "depth": None, "T": None}
+        if len(keep) > ef["n"]:
+            new = [ef["reader"][int(i)] for i in keep[ef["n"]:]]
+            depth = torch.from_numpy(np.stack([x["depth"] for x in new]).astype(np.float32)).to(self.device)
+            T = torch.from_numpy(np.stack([x["T"] for x in new])).float().to(self.device)
+            ef["depth"] = depth if ef["depth"] is None else torch.cat((ef["depth"], depth))
+            ef["T"] = T if ef["T"] is None else torch.cat((ef["T"], T))
+            ef["n"] = len(keep)
+        return ef["depth"][:len(keep)], ef["T"][:len(keep)]
+
+    def _need_gt(self):
+        if self.gt_sdf_interp is None:
+            raise RuntimeError("no ground-truth SDF is loaded: set eval.do_eval and dataset.gt_sdf_dir, or call "
+                               "load_gt_sdf()")
+
+    def eval_sdf(self, samples=200000, visible_region=True):
+        """SDF error against the GT lattice (trainer.py:1815-1866): {'av_l1', 'binned_l1' [6], 'l1_chomp_costs' [3]}
+        as floats.  visible_region: points along rays of the evaluation frames, else uniform in the GT volume.  Points
+        outside the lattice, masked rays and GT values of exactly 0 (wall interiors) are left out; an empty bin is NaN."""
+        self._need_gt()
+        if visible_region:
+            sdf, eval_pts, valid = self._eval_visible(samples)
+        else:
+            (sdf, eval_pts), valid = self.eval_sdf_volume(samples), None
+        gt, inb = self.gt_sdf_interp.sample(eval_pts, fill=1e99)
+        st = self.sdf_map.engine().sdf_error_stats(sdf, gt, inb, valid).cpu().numpy()
+        with np.errstate(invalid="ignore", divide="ignore"):
+            av_l1 = st[1] / st[0]
+            binned = st[8:14] / st[2:8]
+            chomp = st[14:17] / st[0]
+        return {"av_l1": float(av_l1), "binned_l1": [float(v) for v in binned],
+                "l1_chomp_costs": [float(v) for v in chomp]}
+
+    def _eval_visible(self, samples):
+        depth_batch, T_WC_batch = self._eval_frame_data()
+        pts = self.sample_points(depth_batch, T_WC_batch, n_rays=samples // depth_batch.shape[0],
+                                 dist_behind_surf=self.dist_behind_surf, n_strat_samples=1, n_surf_samples=0)
+        with torch.no_grad():
+            sdf = self.sdf_map(pts["pc"], noise_std=0)
+        return sdf.flatten(), pts["pc"].reshape(-1, 3), pts.get("ray_valid")
+
+    def eval_sdf_visible(self, samples=20000):
+        """trainer.py:1868-1905: (sdf [N], points [N,3]) along rays of the evaluation frames (one stratified sample
+        per ray).  In fast mode the rays keep their fixed count and invalid-depth rays stay in (see eval_sdf)."""
+        sdf, pts, _ = self._eval_visible(samples)
+        return sdf, pts
+
+    def eval_sdf_volume(self, samples=20000):
+        """trainer.py:1907-1953: (sdf [N], points [N,3] fp32) uniform in the GT lattice's box, drawn on the CPU; for
+        replicaCAD the points inside the stage (stage_sdf > 0) and off the unnavigable islands are kept."""
+        self._need_gt()
+        eval_pts = torch.rand(samples, 3)
+        eval_pts = eval_pts * (self.sdf_dims - 1)
+        eval_pts = eval_pts * self.sdf_transform[0, 0]
+        eval_pts = eval_pts + torch.from_numpy(self.sdf_transform[:3, 3])
+        if self.dataset_format == "replicaCAD":
+            if self.stage_sdf_interp is None:
+                self.stage_sdf_interp = self._upload_lattice(np.load(self.stage_sdf_file),
+                                                             np.loadtxt(self.sdf_transf_file))
+            eval_pts = eval_pts[torch.from_numpy(self.stage_sdf_interp(eval_pts) > 0)]
+            min_xy = np.loadtxt(self.seq_dir + 'bounds.txt')
+            islands = np.loadtxt(self.seq_dir + 'unnavigable.txt')
+            px = torch.floor((eval_pts[:, 0] - min_xy[0]) / min_xy[2])
+            py = torch.floor((eval_pts[:, 2] - min_xy[1]) / min_xy[2])
+            px = torch.clamp(px, min=0, max=islands.shape[1] - 1).int().numpy()
+            py = torch.clamp(py, min=0, max=islands.shape[0] - 1).int().numpy()
+            eval_pts = eval_pts[torch.from_numpy(islands[py, px] == 0)]
+        with torch.no_grad():
+            eval_pts = eval_pts.float().to(self.device)
+            sdf = self.sdf_map(eval_pts).reshape(-1)
+        return sdf, eval_pts
+
+    def eval_object_sdf(self, samples=10000):
+        """Mean |sdf - gt| in a box around each object of <seq_dir>/obj_bounds.txt (trainer.py:1955-2008): a list with
+        one float per object, NaN for an object not yet seen (at most half of 100 random points of its box visible
+        from the evaluation frames within 5 cm); None without obj_bounds.txt."""
+        if self.obj_bounds_file is None:
+            return None
+        self._need_gt()
+        ob = np.loadtxt(self.obj_bounds_file).reshape(-1, 2, 3)
+        ob[:, 1] += 0.08                                  # metrics.get_obj_eval_bounds: 8 cm around and above
+        ob[:, 0, :self.up_ix] -= 0.08
+        ob[:, 0, self.up_ix + 1:] -= 0.08
+        obj_bounds = torch.FloatTensor(ob).to(self.device)
+        rd = self.rng_device or self.device
+        offsets = torch.rand(100, 3, device=rd).to(self.device)
+        extents = obj_bounds[:, 1] - obj_bounds[:, 0]
+        pts = obj_bounds[:, 0] + offsets[:, None] * extents
+        depth_batch, T_WC_batch = self._eval_frame_data()
+        T_CW = torch.linalg.inv(T_WC_batch)
+        eng = self.sdf_map.engine()
+        visible = eng.points_visible(pts.view(-1, 3), T_CW, depth_batch, self.fx, self.fy, self.cx, self.cy, trunc=0.05)
+        visible = (visible.view(100, len(obj_bounds)).sum(dim=0).cpu().numpy() / 100) > 0.5
+        errors = []
+        for i in range(len(obj_bounds)):
+            if not visible[i]:
+                errors.append(float("nan"))
+                continue
+            offsets = torch.rand(samples, 3, device=rd).to(self.device)
+            bounds = obj_bounds[i]
+            pts = bounds[0] + offsets * (bounds[1] - bounds[0])[None, :]
+            gt, inb = self.gt_sdf_interp.sample(pts, fill=1e99)
+            with torch.no_grad():
+                sdf = self.sdf_map(pts).reshape(-1)
+            keep = inb.bool()
+            errors.append(float((gt[keep] - sdf[keep].double()).abs().mean()))
+        return errors
