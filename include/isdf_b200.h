@@ -338,6 +338,30 @@ int isdfb_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const floa
                          int32_t n_frames, int32_t H, int32_t W, float fx, float fy, float cx, float cy, float trunc,
                          uint8_t* vis, void* stream);
 
+/* ---- the fixed-point evaluation (Trainer.eval_fixed, eval_pts.fixed_pts_eval) -----------------------------------
+ * isdfb_gt_sdf_grad: eval_pts.eval_grad(is_gt_sdf=True) (eval_pts.py:68-93) on the lattice of isdfb_gt_sdf_sample (same
+ *   arguments and checks).  Per point and axis i the two lookups at the point (widened to fp64) plus -delta and +delta
+ *   on axis i, added in fp64, each with isdfb_gt_sdf_sample's arithmetic; a lookup outside the lattice or exactly 0
+ *   becomes NaN; grad_i = ((0 + (-1) s-) + s+) / (2 delta).  grad [n,3] fp64, valid [n] = 1 iff no component is NaN
+ *   (device).  delta > 0.                                                                                           */
+int isdfb_gt_sdf_grad(isdfb_ctx* ctx, const float* lattice, int32_t nx, int32_t ny, int32_t nz,
+                      const double* origin /*[3], host*/, const double* spacing /*[3], host*/, const float* pts_f32,
+                      const double* pts_f64, int64_t n, double delta, double* grad, uint8_t* valid, void* stream);
+
+/* isdfb_sdf_split_stats: the sums of eval_pts.sub_eval (eval_pts.py:18-65): isdfb_sdf_error_stats's 17 sums with no
+ *   point left out (no bounds, validity or zero-GT exclusion: out-of-bounds points carry their fill value), over [0, n)
+ *   in out[0..16] and over [0, n_vox) in out[17..33] (device, fp64), in one pass.  pred fp32 [n], gt fp64 [n];
+ *   0 <= n_vox <= n.  Fixed grid and reduction order: two calls agree bitwise.                                         */
+int isdfb_sdf_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, int64_t n, int64_t n_vox, double* out,
+                          void* stream);
+
+/* isdfb_grad_cosdist: the sum over k < n of 1 - cos(pred[k], gt[r]) with r = gt_index[k] (or k when gt_index is NULL),
+ *   cos as torch.nn.CosineSimilarity(dim=1, eps) on the fp32 prediction and the fp64 GT: each vector divided by its
+ *   2-norm clamped below at eps in its own dtype, the quotients' products in fp64 summed in order (a NaN stays NaN).  pred fp32 [n,3],
+ *   gt fp64 [*,3], gt_index int64 [n] (optional), out [1] fp64 (device).  Fixed reduction order: bitwise repeatable.  */
+int isdfb_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* gt_index, int64_t n,
+                       double eps, double* out, void* stream);
+
 /* ---- kernel timing (bench.py roofline) ---------------------------------------------------
  * When enabled, the tensor-core path brackets its two kernels (the fused PE+MLP chain kernel and
  * the weight-gradient kernel) with CUDA events on the launching stream.  isdfb_profile_read

@@ -486,6 +486,38 @@ int isdfb_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const floa
   return eval_points_visible(ctx, pts, n, T_CW, depth, n_frames, H, W, fx, fy, cx, cy, trunc, vis, st);
 }
 
+int isdfb_gt_sdf_grad(isdfb_ctx* ctx, const float* lattice, int32_t nx, int32_t ny, int32_t nz, const double* origin,
+                      const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double delta,
+                      double* grad, uint8_t* valid, void* stream) {
+  ENTER(ctx);
+  if (!origin || !spacing || n < 0 || (n > 0 && (!lattice || !grad || !valid || (!pts_f32 == !pts_f64))))
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: null argument (or both / neither point arrays)");
+  if (nx < 2 || ny < 2 || nz < 2)
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: lattice %dx%dx%d needs >= 2 nodes per axis", nx, ny, nz);
+  for (int d = 0; d < 3; ++d)
+    if (!(spacing[d] > 0.0) || !isfinite(origin[d]) || !isfinite(spacing[d]))
+      ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: axis %d origin %g spacing %g", d, origin[d], spacing[d]);
+  if (!(delta > 0.0) || !isfinite(delta)) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: delta %g", delta);
+  return eval_gt_grad(ctx, lattice, nx, ny, nz, origin, spacing, pts_f32, pts_f64, n, delta, grad, valid, st);
+}
+
+int isdfb_sdf_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, int64_t n, int64_t n_vox, double* out,
+                          void* stream) {
+  ENTER(ctx);
+  if (!out || n < 0 || (n > 0 && (!pred || !gt))) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_sdf_split_stats: null argument");
+  if (n_vox < 0 || n_vox > n)
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_sdf_split_stats: n_vox %lld outside [0, n = %lld]", (long long)n_vox, (long long)n);
+  return eval_split_stats(ctx, pred, gt, n, n_vox, out, st);
+}
+
+int isdfb_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* gt_index, int64_t n,
+                       double eps, double* out, void* stream) {
+  ENTER(ctx);
+  if (!out || n < 0 || (n > 0 && (!pred || !gt))) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_grad_cosdist: null argument");
+  if (!(eps > 0.0)) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_grad_cosdist: eps %g", eps);
+  return eval_grad_cosdist(ctx, pred, gt, gt_index, n, eps, out, st);
+}
+
 int isdfb_debug_mc_table(uint8_t* rows, int32_t* max_tris) {
   NvtxScope _nvtx(__func__);
   if (!rows && !max_tris) return ISDFB_ERR_ARG;

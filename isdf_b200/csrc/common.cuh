@@ -69,7 +69,7 @@ struct isdfb_ctx {
   float* grid_x;           // fp32 path: lattice points of one chunk (isdfb_mlp_forward_grid), allocated on first use
   void* sample_dev;        // device FusedSampleState {step, valid, blocks_done} of the fused fast-mode sampler
   void* mesh;              // mesh extraction workspace (mesh.cu), created by the first isdfb_mesh_* call, grows on demand
-  void* eval;              // per-block partial sums of isdfb_sdf_error_stats (eval.cu), allocated on first use
+  void* eval;              // per-block partial sums of the eval.cu reductions, allocated on first use
 };
 
 extern char g_isdfb_create_err[512];
@@ -131,3 +131,10 @@ int eval_error_stats(isdfb_ctx* ctx, const float* pred, const double* gt, const 
 int eval_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float* T_CW, const float* depth,
                         int n_frames, int H, int W, float fx, float fy, float cx, float cy, float trunc, uint8_t* vis,
                         cudaStream_t st);
+int eval_gt_grad(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz, const double* origin,
+                 const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double delta,
+                 double* grad, uint8_t* valid, cudaStream_t st);
+int eval_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, int64_t n, int64_t n_vox, double* out,
+                     cudaStream_t st);
+int eval_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* idx, int64_t n, double eps,
+                      double* out, cudaStream_t st);

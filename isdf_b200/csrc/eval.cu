@@ -1,5 +1,5 @@
-// Evaluation against a ground-truth SDF (Trainer.eval_sdf / eval_object_sdf / load_gt_sdf, reference
-// trainer.py:446-453, 1815-2008): three independent kernels.
+// Evaluation against a ground-truth SDF (Trainer.eval_sdf / eval_object_sdf / load_gt_sdf / eval_fixed, reference
+// trainer.py:446-453, 1815-2008, 2080-2087, eval/eval_pts.py): independent kernels.
 //
 // gt_sample_kernel   trilinear interpolation of a resident fp32 [nx,ny,nz] lattice, one thread per point, in the
 //                    arithmetic of scipy's RegularGridInterpolator (method "linear") over the axes
@@ -15,6 +15,12 @@
 //                    GT cost in fp64, as the reference's dtypes); a fixed grid accumulates per thread, reduces per block
 //                    by shuffles in a fixed pattern and writes per-block partials; stats_final_kernel adds the partials
 //                    in block order.  The block count depends on n only, so two calls agree bitwise.
+// gt_grad_kernel     eval_pts.eval_grad(is_gt_sdf=True): six lookups per point with gt_sample_kernel's arithmetic
+//                    (gt_lookup), central differences in eval_grad's order, NaN outside the lattice and at GT zeros.
+// split_stats_kernel eval_pts.sub_eval's sums: stats_kernel's 17 sums with nothing excluded, over [0, n) and [0, n_vox)
+//                    in one pass, on the same fixed grid and in the same fixed order.
+// cosdist_kernel     the sum of 1 - torch.nn.CosineSimilarity(dim=1, eps) over pairs of fp32 predicted and fp64 GT
+//                    gradients, the GT row optionally through an index list; fixed grid and order as stats_kernel.
 // visible_kernel     geometry.frustum.is_visible_torch reduced over the frames (trainer.py:1976-1983): per point and
 //                    frame the fp32 projection with T_CW, 0 < u < W, 0 < v < H, the pixel (int64)(u, v), and
 //                    0 < z < depth + trunc; one byte per point, 1 iff any frame sees it.
@@ -45,25 +51,17 @@ __device__ __forceinline__ int cell(const Axis& a, double x, double* t) {
   return i;
 }
 
-template <typename P>
-__global__ void gt_sample_kernel(const float* __restrict__ lat, Axis ax, Axis ay, Axis az,
-                                 const P* __restrict__ pts, int64_t n, double fill, double* __restrict__ out,
-                                 uint8_t* __restrict__ inb) {
-  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n) return;
-  const double x = (double)pts[3 * p], y = (double)pts[3 * p + 1], z = (double)pts[3 * p + 2];
+// one lookup in the arithmetic described above; *inb is 0 outside the lattice (value `fill`), 1 otherwise
+__device__ __forceinline__ double gt_lookup(const float* __restrict__ lat, const Axis& ax, const Axis& ay,
+                                            const Axis& az, double x, double y, double z, double fill, bool* inb) {
   if (isnan(x) || isnan(y) || isnan(z)) {
-    out[p] = __longlong_as_double(0x7ff8000000000000LL);
-    inb[p] = 1;
-    return;
+    *inb = true;
+    return __longlong_as_double(0x7ff8000000000000LL);
   }
   const bool oob = x < ax.o || x > node(ax, ax.n - 1) || y < ay.o || y > node(ay, ay.n - 1) || z < az.o ||
                    z > node(az, az.n - 1);
-  inb[p] = oob ? 0 : 1;
-  if (oob) {
-    out[p] = fill;
-    return;
-  }
+  *inb = !oob;
+  if (oob) return fill;
   double tx, ty, tz;
   const int i = cell(ax, x, &tx), j = cell(ay, y, &ty), k = cell(az, z, &tz);
   const double w[3][2] = {{__dsub_rn(1.0, tx), tx}, {__dsub_rn(1.0, ty), ty}, {__dsub_rn(1.0, tz), tz}};
@@ -76,7 +74,52 @@ __global__ void gt_sample_kernel(const float* __restrict__ lat, Axis ax, Axis ay
     const double wt = __dmul_rn(__dmul_rn(__dmul_rn(1.0, w[0][a]), w[1][b]), w[2][d]);
     v = __dadd_rn(v, __dmul_rn((double)__ldg(base + a * sx + b * sy + d), wt));
   }
-  out[p] = v;
+  return v;
+}
+
+template <typename P>
+__global__ void gt_sample_kernel(const float* __restrict__ lat, Axis ax, Axis ay, Axis az,
+                                 const P* __restrict__ pts, int64_t n, double fill, double* __restrict__ out,
+                                 uint8_t* __restrict__ inb) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  bool in;
+  out[p] = gt_lookup(lat, ax, ay, az, (double)pts[3 * p], (double)pts[3 * p + 1], (double)pts[3 * p + 2], fill, &in);
+  inb[p] = in ? 1 : 0;
+}
+
+// eval_pts.eval_grad(is_gt_sdf=True): per axis i the lookups at x - delta e_i and x + delta e_i (coordinates widened to
+// fp64, the offset added in fp64; the other two coordinates plus 0.0, i.e. unchanged), a lookup outside the lattice or
+// exactly 0 becomes NaN, grad_i = ((0 + (-1) s-) + s+) / (2 delta); valid = no component NaN (eval_grad's mask)
+template <typename P>
+__global__ void __launch_bounds__(EV_THREADS) gt_grad_kernel(const float* __restrict__ lat, Axis ax, Axis ay, Axis az,
+                                                             const P* __restrict__ pts, int64_t n, double delta,
+                                                             double* __restrict__ grad, uint8_t* __restrict__ valid) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const double c[3] = {(double)pts[3 * p], (double)pts[3 * p + 1], (double)pts[3 * p + 2]};
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  const double two_delta = __dmul_rn(2.0, delta);
+  bool ok = true;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    double g = 0.0;
+#pragma unroll
+    for (int dx = -1; dx <= 1; dx += 2) {
+      const double off = __dmul_rn((double)dx, delta);
+      double q[3];
+#pragma unroll
+      for (int a = 0; a < 3; ++a) q[a] = __dadd_rn(c[a], a == i ? off : 0.0);
+      bool in;
+      double s = gt_lookup(lat, ax, ay, az, q[0], q[1], q[2], 0.0, &in);
+      if (!in || s == 0.0) s = nan;
+      g = __dadd_rn(g, __dmul_rn((double)dx, s));
+    }
+    g = __ddiv_rn(g, two_delta);
+    ok = ok && !isnan(g);
+    grad[3 * p + i] = g;
+  }
+  valid[p] = ok ? 1 : 0;
 }
 
 // metrics.chomp_cost in fp32 (the prediction) and fp64 (the GT), in the reference's operation order
@@ -150,6 +193,113 @@ __global__ void stats_final_kernel(const double* __restrict__ partials, int n_bl
   out[threadIdx.x] = v;
 }
 
+// the sums of eval_pts.sub_eval (and of the objects' and the volume's parts of fixed_pts_eval): stats_kernel's 17 sums
+// with nothing left out -- out-of-bounds points carry their fill, GT zeros count -- over [0, n) and, in the same pass,
+// over [0, n_vox); partials [block][2][17], added in block order by stats_final_kernel over 34 columns
+__global__ void __launch_bounds__(EV_THREADS) split_stats_kernel(const float* __restrict__ pred,
+                                                                 const double* __restrict__ gt, int64_t n,
+                                                                 int64_t n_vox, double* __restrict__ partials) {
+  const double lim[7] = {-1e99, 0.0, 0.1, 0.2, 0.5, 1.0, 1e99};
+  const float eps_f[3] = {1.f, 1.5f, 2.f};
+  const double eps_d[3] = {1.0, 1.5, 2.0};
+  double acc[2][EV_NSTAT];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int q = 0; q < EV_NSTAT; ++q) acc[h][q] = 0.0;
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
+    const double g = gt[p];
+    const float s = pred[p];
+    const double vox = p < n_vox ? 1.0 : 0.0;
+    double v[EV_NSTAT];
+    const double diff = fabs(__dsub_rn((double)s, g));
+    v[0] = 1.0;
+    v[1] = diff;
+#pragma unroll
+    for (int b = 0; b < 6; ++b) {
+      const bool in = g > lim[b] && g < lim[b + 1];
+      v[2 + b] = in ? 1.0 : 0.0;
+      v[8 + b] = in ? diff : 0.0;
+    }
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+      const float cp = chomp_f(s, eps_f[e], (float)(eps_d[e] / 2.0), (float)(1.0 / (2.0 * eps_d[e])));
+      v[14 + e] = fabs(__dsub_rn((double)cp, chomp_d(g, eps_d[e])));
+    }
+#pragma unroll
+    for (int q = 0; q < EV_NSTAT; ++q) {
+      acc[0][q] = __dadd_rn(acc[0][q], v[q]);
+      if (vox != 0.0) acc[1][q] = __dadd_rn(acc[1][q], v[q]);
+    }
+  }
+  __shared__ double red[EV_THREADS / 32][2 * EV_NSTAT];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int q = 0; q < EV_NSTAT; ++q) {
+      double v = acc[h][q];
+      for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_down_sync(0xFFFFFFFFu, v, o));
+      if (lane == 0) red[warp][h * EV_NSTAT + q] = v;
+    }
+  __syncthreads();
+  if (threadIdx.x < 2 * EV_NSTAT) {
+    double v = 0.0;
+    for (int w = 0; w < EV_THREADS / 32; ++w) v = __dadd_rn(v, red[w][threadIdx.x]);
+    partials[(int64_t)blockIdx.x * 2 * EV_NSTAT + threadIdx.x] = v;
+  }
+}
+
+// the final sum of a fixed grid's partials [block][cols], column by column in block order
+__global__ void partials_final_kernel(const double* __restrict__ partials, int n_blocks, int cols,
+                                      double* __restrict__ out) {
+  if (threadIdx.x >= cols) return;
+  double v = 0.0;
+  for (int b = 0; b < n_blocks; ++b) v = __dadd_rn(v, partials[(int64_t)b * cols + threadIdx.x]);
+  out[threadIdx.x] = v;
+}
+
+// kept out of line: inlined, the fp64 division and square-root slow paths spill the reduction loop's state
+__device__ __noinline__ double cos_sim(const float* __restrict__ p, const double* __restrict__ q, double eps) {
+  const float a0 = p[0], a1 = p[1], a2 = p[2];
+  const double b0 = q[0], b1 = q[1], b2 = q[2];
+  float na = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(a0, a0), __fmul_rn(a1, a1)), __fmul_rn(a2, a2)));
+  double nb = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(b0, b0), __dmul_rn(b1, b1)), __dmul_rn(b2, b2)));
+  const float eps_f = (float)eps;
+  na = na < eps_f ? eps_f : na;                          // clamp_min: a NaN norm stays NaN
+  nb = nb < eps ? eps : nb;
+  const double c0 = __dmul_rn((double)__fdiv_rn(a0, na), __ddiv_rn(b0, nb));
+  const double c1 = __dmul_rn((double)__fdiv_rn(a1, na), __ddiv_rn(b1, nb));
+  const double c2 = __dmul_rn((double)__fdiv_rn(a2, na), __ddiv_rn(b2, nb));
+  return __dadd_rn(__dadd_rn(c0, c1), c2);
+}
+
+// torch.nn.CosineSimilarity(dim=1, eps) on the pair (pred fp32, gt fp64) as torch normalises them: each row divided by
+// its 2-norm clamped below at eps in its own dtype (a NaN norm stays NaN, as clamp_min keeps it), the fp32 quotients
+// promoted to fp64 and the three products summed in order (torch's norm may accumulate the fp32 squares differently:
+// the cosines agree to a few fp32 ulps, not bitwise); the kernel
+// sums 1 - cos over the pairs (gt row idx[k] when an index list is given), per block in a fixed pattern
+__global__ void __launch_bounds__(EV_THREADS) cosdist_kernel(const float* __restrict__ pred,
+                                                             const double* __restrict__ gt,
+                                                             const int64_t* __restrict__ idx, int64_t n, double eps,
+                                                             double* __restrict__ partials) {
+  double acc = 0.0;
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = idx ? idx[k] : k;
+    acc = __dadd_rn(acc, __dsub_rn(1.0, cos_sim(pred + 3 * k, gt + 3 * r, eps)));
+  }
+  __shared__ double red[EV_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int o = 16; o > 0; o >>= 1) acc = __dadd_rn(acc, __shfl_down_sync(0xFFFFFFFFu, acc, o));
+  if (lane == 0) red[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double v = 0.0;
+    for (int w = 0; w < EV_THREADS / 32; ++w) v = __dadd_rn(v, red[w]);
+    partials[blockIdx.x] = v;
+  }
+}
+
 __global__ void visible_kernel(const float* __restrict__ pts, int64_t n, const float* __restrict__ T_CW,
                                const float* __restrict__ depth, int n_frames, int H, int W, float fx, float fy, float cx,
                                float cy, float trunc, uint8_t* __restrict__ vis) {
@@ -197,11 +347,20 @@ int eval_gt_sample(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz,
   return ISDFB_OK;
 }
 
+// ctx->eval: room for the largest partials layout ([block][2][17] of the split statistics)
+static int eval_partials(isdfb_ctx* ctx, double** out) {
+  if (!ctx->eval) ISDFB_CUDA_OK(ctx, cudaMalloc(&ctx->eval, sizeof(double) * EV_STATS_BLOCKS * 2 * EV_NSTAT));
+  *out = (double*)ctx->eval;
+  return ISDFB_OK;
+}
+
+inline int stats_blocks(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(EV_STATS_BLOCKS, blocks_for(n))); }
+
 int eval_error_stats(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, const uint8_t* valid,
                      int64_t n, double* out, cudaStream_t st) {
-  if (!ctx->eval) ISDFB_CUDA_OK(ctx, cudaMalloc(&ctx->eval, sizeof(double) * EV_STATS_BLOCKS * EV_NSTAT));
-  const int nb = (int)std::max<int64_t>(1, std::min<int64_t>(EV_STATS_BLOCKS, blocks_for(n)));
-  double* partials = (double*)ctx->eval;
+  double* partials;
+  if (int rc = eval_partials(ctx, &partials)) return rc;
+  const int nb = stats_blocks(n);
   stats_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, inb, valid, n, partials);
   ISDFB_CUDA_OK(ctx, cudaGetLastError());
   stats_final_kernel<<<1, 32, 0, st>>>(partials, nb, out);
@@ -217,5 +376,46 @@ int eval_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float
   visible_kernel<<<blocks_for(n), EV_THREADS, 0, st>>>(pts, n, T_CW, depth, n_frames, H, W, fx, fy, cx, cy, trunc, vis);
   ISDFB_CUDA_OK(ctx, cudaGetLastError());
   ISDFB_LAUNCHED(ctx);
+  return ISDFB_OK;
+}
+
+int eval_gt_grad(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz, const double* origin,
+                 const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double delta,
+                 double* grad, uint8_t* valid, cudaStream_t st) {
+  if (n == 0) return ISDFB_OK;
+  if ((int64_t)blocks_for(n) > 0x7FFFFFFFLL) ISDFB_FAIL(ctx, ISDFB_ERR_CAPACITY, "isdfb_gt_sdf_grad: %lld points", (long long)n);
+  const Axis ax{origin[0], spacing[0], nx}, ay{origin[1], spacing[1], ny}, az{origin[2], spacing[2], nz};
+  if (pts_f64)
+    gt_grad_kernel<double><<<blocks_for(n), EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts_f64, n, delta, grad, valid);
+  else
+    gt_grad_kernel<float><<<blocks_for(n), EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts_f32, n, delta, grad, valid);
+  ISDFB_CUDA_OK(ctx, cudaGetLastError());
+  ISDFB_LAUNCHED(ctx);
+  return ISDFB_OK;
+}
+
+int eval_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, int64_t n, int64_t n_vox, double* out,
+                     cudaStream_t st) {
+  double* partials;
+  if (int rc = eval_partials(ctx, &partials)) return rc;
+  const int nb = stats_blocks(n);
+  split_stats_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, n, n_vox, partials);
+  ISDFB_CUDA_OK(ctx, cudaGetLastError());
+  partials_final_kernel<<<1, 64, 0, st>>>(partials, nb, 2 * EV_NSTAT, out);
+  ISDFB_CUDA_OK(ctx, cudaGetLastError());
+  ctx->launches += 2;
+  return ISDFB_OK;
+}
+
+int eval_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* idx, int64_t n, double eps,
+                      double* out, cudaStream_t st) {
+  double* partials;
+  if (int rc = eval_partials(ctx, &partials)) return rc;
+  const int nb = stats_blocks(n);
+  cosdist_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, idx, n, eps, partials);
+  ISDFB_CUDA_OK(ctx, cudaGetLastError());
+  partials_final_kernel<<<1, 32, 0, st>>>(partials, nb, 1, out);
+  ISDFB_CUDA_OK(ctx, cudaGetLastError());
+  ctx->launches += 2;
   return ISDFB_OK;
 }

@@ -339,6 +339,63 @@ class Engine:
                                                self._stream()))
         return vis
 
+    def gt_sdf_grad(self, lattice, origin, spacing, pts, delta):
+        """eval_pts.eval_grad(is_gt_sdf=True) on the lattice of gt_sdf_sample at pts [N,3] (float32 or float64): central
+        differences of step delta, NaN where a lookup is outside the lattice or exactly 0.  Returns (grad fp64 [N,3],
+        valid uint8 [N], 1 iff no component is NaN)."""
+        lattice = _f32(lattice, "lattice", self.device)
+        if lattice.dim() != 3:
+            raise ValueError("lattice must be [nx,ny,nz], got %s" % (tuple(lattice.shape),))
+        if (pts.device != self.device or pts.dtype not in (torch.float32, torch.float64) or pts.dim() != 2
+                or pts.shape[1] != 3):
+            raise TypeError("pts must be a float32 or float64 [N,3] tensor on %s" % self.device)
+        pts = pts.contiguous()
+        n = pts.shape[0]
+        grad = torch.empty(n, 3, dtype=torch.float64, device=self.device)
+        valid = torch.empty(n, dtype=torch.uint8, device=self.device)
+        o = (C.c_double * 3)(*[float(v) for v in origin])
+        s = (C.c_double * 3)(*[float(v) for v in spacing])
+        f64 = pts.dtype == torch.float64
+        self._ck(self.lib.isdfb_gt_sdf_grad(self._ctx, _ptr(lattice), *[int(d) for d in lattice.shape], o, s,
+                                            _ptr(None if f64 else pts), _ptr(pts if f64 else None), n, float(delta),
+                                            _ptr(grad), _ptr(valid), self._stream()))
+        return grad, valid
+
+    def sdf_split_stats(self, pred, gt, n_vox):
+        """eval_pts.sub_eval's sums (device fp64 [2,17]): row 0 over all points, row 1 over the first n_vox, each in
+        sdf_error_stats's layout, with no point left out."""
+        pred = _f32(pred, "pred", self.device).reshape(-1)
+        n = pred.numel()
+        if gt.dtype != torch.float64 or gt.device != self.device or gt.numel() != n:
+            raise TypeError("gt must be float64 on %s with one value per prediction" % self.device)
+        if not 0 <= int(n_vox) <= n:
+            raise ValueError("n_vox %d outside [0, %d]" % (n_vox, n))
+        out = torch.empty(2, 17, dtype=torch.float64, device=self.device)
+        self._ck(self.lib.isdfb_sdf_split_stats(self._ctx, _ptr(pred), _ptr(gt.reshape(-1).contiguous()), n,
+                                                int(n_vox), _ptr(out), self._stream()))
+        return out
+
+    def grad_cosdist(self, pred, gt, gt_index=None, eps=1e-6):
+        """Sum over k of 1 - CosineSimilarity(dim=1, eps)(pred[k], gt[gt_index[k]]) (gt[k] without an index), in fp64
+        (device tensor [1]).  pred fp32 [M,3], gt fp64 [N,3], gt_index int64 [M]."""
+        pred = _f32(pred, "pred", self.device)
+        if pred.dim() != 2 or pred.shape[1] != 3:
+            raise ValueError("pred must be [M,3], got %s" % (tuple(pred.shape),))
+        if gt.dtype != torch.float64 or gt.device != self.device or gt.dim() != 2 or gt.shape[1] != 3:
+            raise TypeError("gt must be a float64 [N,3] tensor on %s" % self.device)
+        gt = gt.contiguous()
+        m = pred.shape[0]
+        if gt_index is not None:
+            gt_index = _i64(gt_index, "gt_index", self.device).reshape(-1)
+            if gt_index.numel() != m:
+                raise ValueError("gt_index must have one entry per prediction")
+        elif gt.shape[0] != m:
+            raise ValueError("gt must have one row per prediction without gt_index")
+        out = torch.empty(1, dtype=torch.float64, device=self.device)
+        self._ck(self.lib.isdfb_grad_cosdist(self._ctx, _ptr(pred), _ptr(gt), _ptr(gt_index), m, float(eps), _ptr(out),
+                                             self._stream()))
+        return out
+
     # ---- N2 ----------------------------------------------------------
     def bounds_pc(self, pc, z_vals, depth_sample, ray_valid=None):
         """loss.bounds_pc (loss.py:56-89): bounds [R,S] and target directions [R,S,3] (row 0 unused)."""

@@ -16,7 +16,8 @@ Two RNG modes: "reference" consumes torch / numpy generators in exactly the refe
 "fast" keeps fixed shapes with a validity mask and never synchronises inside the step.
 Visualisation is out of scope (SURVEY.md section 2) and raises; mesh extraction (mesh_rec, write_mesh) runs on the
 device (isdfb_mesh_*), and so does the evaluation against a ground-truth SDF (load_gt_sdf, eval_sdf, eval_object_sdf:
-isdfb_gt_sdf_sample, isdfb_sdf_error_stats, isdfb_points_visible).
+isdfb_gt_sdf_sample, isdfb_sdf_error_stats, isdfb_points_visible; eval_fixed: isdfb_gt_sdf_grad, isdfb_sdf_split_stats,
+isdfb_grad_cosdist).
 """
 import copy
 import json
@@ -36,12 +37,16 @@ from .. import parallel
 from . import embedding, fc_map, render, sample
 
 _OUT_OF_SCOPE = ("view_sdf", "latest_frame_vis", "update_vis_vars", "frames_vis", "draw_3D", "draw_obj_3D",
-                 "obj_slices_vis", "write_slices", "eval_fixed", "eval_mesh", "compute_slices", "keyframe_vis",
+                 "obj_slices_vis", "write_slices", "eval_mesh", "compute_slices", "keyframe_vis",
                  "slices_vis", "render_depth_vis", "render_normals_vis", "to_topdown", "check_gt_sdf", "eval_traj_cost")
 
 # the evaluation frames' depth transform (eval_pts.get_cache_dataset): fixed scale per format, far values zeroed at 12 m
 _EVAL_DEPTH_SCALE = {"replicaCAD": 1. / 3276.75, "ScanNet": 1. / 1000.}
 _EVAL_FRAME_STRIDE = 5
+# eval_pts_dir's voxblox voxel size per frac_time_perception (trainer.py:272-282)
+_VOX_RES_DIR = {1.: "0.055/", 0.75: "0.063/", 0.5: "0.078/", 0.25: "0.11/"}
+# eval_pts.fixed_pts_eval's literals: samples per point set, near limit, central-difference step, objects' samples
+_FIXED_SAMPLES, _FIXED_MIN_DEPTH, _FIXED_GRAD_DELTA, _FIXED_OBJ_SAMPLES = 200000, 0.1, 0.01, 10000
 
 
 class GtSdfInterp:
@@ -299,10 +304,17 @@ class Trainer:
             raise NotImplementedError("gaussian / optimised embeddings are not used by any shipped config")
 
         ev = cfg["eval"]
-        self.do_vox_comparison = bool(ev["do_vox_comparison"]) and "eval_pts_root" in ev and False
+        self.do_vox_comparison = bool(ev["do_vox_comparison"]) and "eval_pts_root" in ev
         self.do_eval, self.eval_freq_s = ev["do_eval"], ev["eval_freq_s"]
         self.sdf_eval, self.mesh_eval = bool(ev["sdf_eval"]), bool(ev["mesh_eval"])
         self.eval_times = []
+        if self.do_vox_comparison:                     # trainer.py:268-290: the voxblox comparison's fixed points
+            if self.frac_time_perception not in _VOX_RES_DIR:
+                raise ValueError("Frace perception time not in [0.25, 0.5, 0.75, 1.]")
+            self.eval_pts_root = ev["eval_pts_root"]
+            self.eval_pts_dir = (self.eval_pts_root + "/vox/" + _VOX_RES_DIR[self.frac_time_perception]
+                                 + [x for x in self.seq_dir.split('/') if x != ""][-1] + "/eval_pts/")
+            self.eval_times = sorted(float(x) for x in os.listdir(self.eval_pts_dir))
         sv = cfg["save"]
         self.save_period = sv["save_period"]
         self.save_times = np.arange(self.save_period, 2000, self.save_period).tolist()
@@ -1098,15 +1110,23 @@ class Trainer:
         """The evaluation frames of eval_pts.get_cache_dataset: every 5th frame of the sequence, read with the fixed
         depth scale of the format and a 12 m cut (no noisy depth); incremental runs see the frames before
         int(tot_step_time * fps).  Kept on the device and extended as the run advances.  (depth [F,H,W], T_WC [F,4,4])"""
+        depth, T_WC = self._eval_frames_before(int(self.tot_step_time * self.fps) if self.incremental else None)
+        if depth is None:
+            raise RuntimeError("no evaluation frame yet: the run has not reached frame 0 (tot_step_time %g s)"
+                               % self.tot_step_time)
+        return depth, T_WC
+
+    def _eval_frames_before(self, limit):
+        """The evaluation frames with index < limit (all with limit None), from the device cache that _eval_frame_data
+        describes; (None, None) when there is none."""
         if self.dataset_format not in _EVAL_DEPTH_SCALE:
             raise NotImplementedError("evaluation frames are defined for the replicaCAD and ScanNet formats only, "
                                       "not %r" % self.dataset_format)
         keep = np.arange(0, len(self.scene_dataset), _EVAL_FRAME_STRIDE)
-        if self.incremental:
-            keep = keep[keep < int(self.tot_step_time * self.fps)]
+        if limit is not None:
+            keep = keep[keep < limit]
         if len(keep) == 0:
-            raise RuntimeError("no evaluation frame yet: the run has not reached frame 0 (tot_step_time %g s)"
-                               % self.tot_step_time)
+            return None, None
         ef = self._eval_frames
         if ef is None:
             tf = ds.depth_scale_filter(_EVAL_DEPTH_SCALE[self.dataset_format], 12.0)
@@ -1221,3 +1241,153 @@ class Trainer:
             keep = inb.bool()
             errors.append(float((gt[keep] - sdf[keep].double()).abs().mean()))
         return errors
+
+    # ---- the voxblox comparison's fixed-point evaluation (trainer.py:2080-2087, eval/eval_pts.py:96-299) -----------
+    def eval_fixed(self):
+        """eval_pts.fixed_pts_eval at the next of eval_times, which it pops: the map scored on the point sets whose
+        masks were precomputed for the voxblox comparison (<eval_pts_dir>/<t>/*.npy).  Returns the dict of one
+        vox_res.json entry with plain floats (NaN for an empty set):
+          time
+          rays          {vis, vox}: av_l1, binned_l1 [6], l1_chomp_costs [3], av_cossim [2]
+          visible_surf  {vis, vox}: av_l1, binned_l1, l1_chomp_costs
+          objects       [{vis: {av_l1}, vox: {av_l1}}] for the objects with mask files (only with obj_bounds.txt)
+          vol           av_l1, binned_l1, l1_chomp_costs
+        The points are the reference's own: torch's CPU generator reseeded from t draws the pixels and depths, numpy's
+        global generator the object points, and both are left as the reference leaves them.  Nothing else changes."""
+        t = self.eval_times.pop(0)
+        return self._fixed_pts_eval(t)
+
+    def _fixed_mask(self, masks_dir, name, length=None):
+        path = masks_dir + "/" + name + ".npy"
+        m = np.load(path)
+        if m.dtype != np.bool_ or m.ndim != 1:
+            raise ValueError("%s: expected a 1-D boolean mask, got %s %s" % (path, m.dtype, m.shape))
+        if length is not None and len(m) != length:
+            raise ValueError("%s: %d entries for %d points" % (path, len(m), length))
+        return m
+
+    def _fixed_pts_eval(self, t):
+        self._need_gt()
+        eng = self.sdf_map.engine()
+        dev = self.device
+        t_str = f"{t:.3f}"
+        pts_dir = os.path.join(self.eval_pts_dir, t_str)
+        masks_dir = self.eval_pts_dir + t_str
+        depth, T_WC = self._eval_frames_before(min(np.floor(t * 30), len(self.scene_dataset)))
+        if depth is None:
+            raise RuntimeError("no evaluation frame before t = %s s" % t_str)
+        if tuple(depth.shape[1:]) != (self.H, self.W):
+            raise ValueError("evaluation frames are %s, the camera is %dx%d" % (tuple(depth.shape[1:]), self.H, self.W))
+        n_frames = depth.shape[0]
+
+        # sample_rays (eval_pts.py:354-400), whose depth_batch is a CPU tensor: every call reseeds torch from t and
+        # draws the pixels, then the visible-region calls draw one stratified depth per ray, all on the CPU generator.
+        # The two visible-region calls draw the same points, and the surface call the same pixels: K1 computes both sets
+        # in one launch (sample 0 on the surface, sample 1 stratified), and the surface call's draws are repeated last.
+        seed = float(t_str) * 1e3
+        rays_per_frame = _FIXED_SAMPLES // n_frames
+        torch.manual_seed(seed)
+        ib, ih, iw = [x.to(dev) for x in sample.sample_pixels(rays_per_frame, n_frames, self.H, self.W, device="cpu")]
+        depth_s, _, valid = eng.gather_rays(depth, None, ib, ih, iw, self.cam)
+        keep = valid.bool()
+        depth_s, ib, ih, iw = depth_s[keep], ib[keep], ih[keep], iw[keep]
+        n = depth_s.shape[0]
+        u = torch.rand(n, 1).to(dev)
+        dist_behind = 0. if self.dataset_format == "ScanNet" else 0.1
+        pc, _, _, _ = eng.sample_rays(T_WC, ib, ih, iw, depth_s, u, None, self._lin(1), 1, 1, self.cam,
+                                      _FIXED_MIN_DEPTH, dist_behind)
+        surf_pts, vis_pts = pc[:, 0].contiguous(), pc[:, 1].contiguous()
+        torch.manual_seed(seed)
+        sample.sample_pixels(rays_per_frame, n_frames, self.H, self.W, device="cpu")
+
+        names = ("surf_valid_gt_sdf", "vis_valid_gt_sdf", "vis_valid_gt_grad")
+        m = {k: self._fixed_mask(masks_dir, k, n) for k in names}
+        for k in names:
+            vox = k.replace("_gt_", "_vox_")
+            m[vox] = self._fixed_mask(masks_dir, vox)
+            if m[k].sum() != len(m[vox]):                # eval_pts.py:122-124
+                raise ValueError("%s/%s.npy: %d entries for the %d points %s selects"
+                                 % (masks_dir, vox, len(m[vox]), m[k].sum(), k))
+        md = {k: torch.from_numpy(v).to(dev) for k, v in m.items()}
+        stats, cos, counts = [], [], []
+
+        def split(pts, gt_mask, vox_mask):
+            """sub_eval's order (eval_pts.py:18-65): the points gt_mask selects, those in vox_mask first."""
+            sel = gt_mask.nonzero().squeeze(1)
+            idx = torch.cat((sel[vox_mask], sel[~vox_mask]))
+            return pts[idx], int(vox_mask.sum()), sel
+
+        def sub_eval(pts, n_vox):
+            gt, _ = self.gt_sdf_interp.sample(pts, fill=1e99)          # eval_sdf_interp(handle_oob='mask')
+            pred = eng.forward(pts.float()) if len(pts) else torch.empty(0, device=dev)
+            stats.append(eng.sdf_split_stats(pred, gt, n_vox))
+
+        # rays: the visible region's points and the GT gradient (central differences of 1 cm) at every one of them
+        pts, n_vox, sel = split(vis_pts, md["vis_valid_gt_sdf"], md["vis_valid_vox_sdf"])
+        sub_eval(pts, n_vox)
+        gti = self.gt_sdf_interp
+        gt_grad, _ = eng.gt_sdf_grad(gti.lattice, gti.origin, gti.spacing, vis_pts, _FIXED_GRAD_DELTA)
+        vis_idx = md["vis_valid_gt_grad"].nonzero().squeeze(1)
+        vox_idx = sel[md["vis_valid_vox_sdf"]]
+        vox_idx = vox_idx[md["vis_valid_gt_grad"][vox_idx]]
+        for idx in (vis_idx, vox_idx):                   # grad_fn: K3's d sdf / dx
+            pred = eng.forward(vis_pts[idx], want_grad=True)[1] if len(idx) else torch.empty(0, 3, device=dev)
+            cos.append(eng.grad_cosdist(pred, gt_grad, idx))
+            counts.append(idx.numel())
+
+        pts, n_vox, _ = split(surf_pts, md["surf_valid_gt_sdf"], md["surf_valid_vox_sdf"])
+        sub_eval(pts, n_vox)
+
+        obj_ix = []
+        if self.obj_bounds_file is not None:
+            obj_bounds = np.loadtxt(self.obj_bounds_file).reshape(-1, 2, 3)
+            obj_bounds[:, 1] += 0.08                     # eval_pts.load_obj_bounds: x and z widened, whatever is up
+            obj_bounds[:, 0, 0] -= 0.08
+            obj_bounds[:, 0, 2] -= 0.08
+            files = os.listdir(pts_dir)
+            for i, bounds in enumerate(obj_bounds):
+                if not any(f"obj{i}" in x for x in files):  # a substring test: obj1 also matches obj10's files
+                    continue
+                gt_mask = self._fixed_mask(masks_dir, f"obj{i}_valid_gt_sdf", _FIXED_OBJ_SAMPLES)
+                vox_mask = self._fixed_mask(masks_dir, f"obj{i}_valid_vox_sdf", int(gt_mask.sum()))
+                np.random.seed(0)                        # eval_pts.object_eval_pts
+                offsets = torch.from_numpy(np.random.rand(_FIXED_OBJ_SAMPLES, 3)).to(dev)
+                b = torch.from_numpy(bounds).to(dev)
+                pts = b[0] + offsets * (b[1] - b[0])[None, :]
+                pts, n_vox, _ = split(pts, torch.from_numpy(gt_mask).to(dev), torch.from_numpy(vox_mask).to(dev))
+                sub_eval(pts, n_vox)
+                obj_ix.append(len(stats) - 1)
+
+        # the volume: its own points and GT values, every point counted
+        root, seq = self.eval_pts_root, [x for x in self.seq_dir.split('/') if x != ""][-1]
+        vol_file = root + ("full_vol/replicaCAD.npy" if self.dataset_format == "replicaCAD" else f"full_vol/{seq}.npy")
+        vol_pts = torch.from_numpy(np.load(vol_file).reshape(-1, 3)).to(dev)
+        vol_gt = torch.from_numpy(np.load(root + f"full_vol/gt_{seq}.npy").astype(np.float64).reshape(-1)).to(dev)
+        if vol_gt.numel() != vol_pts.shape[0]:
+            raise ValueError("full_vol/gt_%s.npy: %d values for %d points" % (seq, vol_gt.numel(), vol_pts.shape[0]))
+        stats.append(eng.sdf_split_stats(eng.forward(vol_pts.float()), vol_gt, 0))
+
+        st = torch.stack(stats).cpu().numpy()            # [parts, 2, 17]
+        cs = torch.cat(cos).cpu().numpy()
+        with np.errstate(invalid="ignore", divide="ignore"):
+            cosdist = [float(c / k) for c, k in zip(cs, counts)]
+        rays = _split_result(st[0])
+        rays["vis"]["av_cossim"] = [cosdist[0], cosdist[0]]      # vis_grad_2 = vis_grad_1
+        rays["vox"]["av_cossim"] = [cosdist[1], cosdist[1]]      # the reference stores vox_1 twice
+        res = {"time": t, "rays": rays, "visible_surf": _split_result(st[1])}
+        if self.obj_bounds_file is not None:
+            res["objects"] = [{h: {"av_l1": _stats_result(st[i][r])["av_l1"]} for r, h in enumerate(("vis", "vox"))}
+                              for i in obj_ix]
+        res["vol"] = _stats_result(st[-1][0])
+        return res
+
+
+def _stats_result(st):
+    """{'av_l1', 'binned_l1', 'l1_chomp_costs'} as floats from the 17 sums of isdfb_sdf_split_stats (0 / 0 = NaN)."""
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return {"av_l1": float(st[1] / st[0]), "binned_l1": [float(v) for v in st[8:14] / st[2:8]],
+                "l1_chomp_costs": [float(v) for v in st[14:17] / st[0]]}
+
+
+def _split_result(st):
+    return {"vis": _stats_result(st[0]), "vox": _stats_result(st[1])}
