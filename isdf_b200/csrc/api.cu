@@ -78,6 +78,21 @@ static int build_layout(const isdfb_model_cfg& cfg, ModelLayout* lay, char* err,
   return ISDFB_OK;
 }
 
+// the lattice, point and output arguments of isdfb_gt_sdf_sample and isdfb_gt_sdf_grad; `entry` names the entry in
+// the message
+static int check_lattice(isdfb_ctx* ctx, const char* entry, const float* lattice, int32_t nx, int32_t ny, int32_t nz,
+                         const double* origin, const double* spacing, const float* pts_f32, const double* pts_f64,
+                         int64_t n, const void* out, const uint8_t* out_mask) {
+  if (!origin || !spacing || n < 0 || (n > 0 && (!lattice || !out || !out_mask || (!pts_f32 == !pts_f64))))
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "%s: null argument (or both / neither point arrays)", entry);
+  if (nx < 2 || ny < 2 || nz < 2)
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "%s: lattice %dx%dx%d needs >= 2 nodes per axis", entry, nx, ny, nz);
+  for (int d = 0; d < 3; ++d)
+    if (!(spacing[d] > 0.0) || !isfinite(origin[d]) || !isfinite(spacing[d]))
+      ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "%s: axis %d origin %g spacing %g", entry, d, origin[d], spacing[d]);
+  return ISDFB_OK;
+}
+
 extern "C" {
 
 int isdfb_create(const isdfb_model_cfg* cfg, int device, isdfb_ctx** out) {
@@ -457,13 +472,8 @@ int isdfb_gt_sdf_sample(isdfb_ctx* ctx, const float* lattice, int32_t nx, int32_
                         const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double fill,
                         double* out, uint8_t* in_bounds, void* stream) {
   ENTER(ctx);
-  if (!origin || !spacing || n < 0 || (n > 0 && (!lattice || !out || !in_bounds || (!pts_f32 == !pts_f64))))
-    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_sample: null argument (or both / neither point arrays)");
-  if (nx < 2 || ny < 2 || nz < 2)
-    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_sample: lattice %dx%dx%d needs >= 2 nodes per axis", nx, ny, nz);
-  for (int d = 0; d < 3; ++d)
-    if (!(spacing[d] > 0.0) || !isfinite(origin[d]) || !isfinite(spacing[d]))
-      ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_sample: axis %d origin %g spacing %g", d, origin[d], spacing[d]);
+  if (int rc = check_lattice(ctx, __func__, lattice, nx, ny, nz, origin, spacing, pts_f32, pts_f64, n, out, in_bounds))
+    return rc;
   return eval_gt_sample(ctx, lattice, nx, ny, nz, origin, spacing, pts_f32, pts_f64, n, fill, out, in_bounds, st);
 }
 
@@ -490,13 +500,8 @@ int isdfb_gt_sdf_grad(isdfb_ctx* ctx, const float* lattice, int32_t nx, int32_t 
                       const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double delta,
                       double* grad, uint8_t* valid, void* stream) {
   ENTER(ctx);
-  if (!origin || !spacing || n < 0 || (n > 0 && (!lattice || !grad || !valid || (!pts_f32 == !pts_f64))))
-    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: null argument (or both / neither point arrays)");
-  if (nx < 2 || ny < 2 || nz < 2)
-    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: lattice %dx%dx%d needs >= 2 nodes per axis", nx, ny, nz);
-  for (int d = 0; d < 3; ++d)
-    if (!(spacing[d] > 0.0) || !isfinite(origin[d]) || !isfinite(spacing[d]))
-      ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: axis %d origin %g spacing %g", d, origin[d], spacing[d]);
+  if (int rc = check_lattice(ctx, __func__, lattice, nx, ny, nz, origin, spacing, pts_f32, pts_f64, n, grad, valid))
+    return rc;
   if (!(delta > 0.0) || !isfinite(delta)) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_gt_sdf_grad: delta %g", delta);
   return eval_gt_grad(ctx, lattice, nx, ny, nz, origin, spacing, pts_f32, pts_f64, n, delta, grad, valid, st);
 }

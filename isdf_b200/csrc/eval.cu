@@ -10,17 +10,18 @@
 //                    rounded on its own (no contraction).  Out of bounds (x < grid[0] or x > grid[-1] on any axis) gives
 //                    the fill value; a NaN coordinate gives NaN and counts as in bounds, as scipy's NaN pass overwrites
 //                    the fill (so the byte equals sdf_util.eval_sdf_interp's mask).  Corners are widened to fp64.
-// stats_kernel       the reduction of eval_sdf (trainer.py:1831-1864, metrics.binned_losses, metrics.chomp_cost):
-//                    per point the fp64 |pred - gt|, its bin and the three CHOMP differences (prediction cost in fp32,
-//                    GT cost in fp64, as the reference's dtypes); a fixed grid accumulates per thread, reduces per block
-//                    by shuffles in a fixed pattern and writes per-block partials; stats_final_kernel adds the partials
-//                    in block order.  The block count depends on n only, so two calls agree bitwise.
 // gt_grad_kernel     eval_pts.eval_grad(is_gt_sdf=True): six lookups per point with gt_sample_kernel's arithmetic
 //                    (gt_lookup), central differences in eval_grad's order, NaN outside the lattice and at GT zeros.
-// split_stats_kernel eval_pts.sub_eval's sums: stats_kernel's 17 sums with nothing excluded, over [0, n) and [0, n_vox)
-//                    in one pass, on the same fixed grid and in the same fixed order.
+// stats_kernel<ROWS> the 17 sums of the SDF error (metrics.binned_losses, metrics.chomp_cost): per point the fp64
+//                    |pred - gt|, its bin and the three CHOMP differences (prediction cost in fp32, GT cost in fp64, as
+//                    the reference's dtypes), all from point_stats.  ROWS = 1 is eval_sdf (trainer.py:1831-1864), which
+//                    leaves out points outside the lattice, masked out or with gt == 0; ROWS = 2 is eval_pts.sub_eval,
+//                    which keeps every point and sums [0, n) and [0, n_vox) in one pass.
 // cosdist_kernel     the sum of 1 - torch.nn.CosineSimilarity(dim=1, eps) over pairs of fp32 predicted and fp64 GT
-//                    gradients, the GT row optionally through an index list; fixed grid and order as stats_kernel.
+//                    gradients, the GT row optionally through an index list.
+// partials_final_kernel  the last step of stats_kernel's and cosdist_kernel's reduction: on a grid fixed by n, each
+//                    thread accumulates, block_partials reduces each block by shuffles in a fixed pattern, and this
+//                    kernel adds the per-block partials in block order.  So two calls on the same input agree bitwise.
 // visible_kernel     geometry.frustum.is_visible_torch reduced over the frames (trainer.py:1976-1983): per point and
 //                    frame the fp32 projection with T_CW, 0 < u < W, 0 < v < H, the pixel (int64)(u, v), and
 //                    0 < z < depth + trunc; one byte per point, 1 iff any frame sees it.
@@ -140,114 +141,73 @@ __device__ __forceinline__ double chomp_d(double s, double eps) {
   return __dadd_rn(-s, eps / 2.0);
 }
 
-// layout of the 17 sums: [0] count, [1] sum |pred - gt|, [2..7] bin counts, [8..13] bin sums, [14..16] CHOMP sums
-__global__ void __launch_bounds__(EV_THREADS) stats_kernel(const float* __restrict__ pred, const double* __restrict__ gt,
-                                                           const uint8_t* __restrict__ inb,
-                                                           const uint8_t* __restrict__ valid, int64_t n,
-                                                           double* __restrict__ partials) {
+// the 17 values one (prediction, GT) pair adds to the sums, passed to add(q, value): [0] count, [1] |pred - gt|,
+// [2..7] bin counts, [8..13] bin sums, [14..16] CHOMP differences; the bins are open intervals between the edges.
+// Each value goes to `add` as soon as it is computed: collected in an array first, stats_kernel<1> is scheduled ~2%
+// slower and stats_kernel<2> needs 119 registers instead of 92.
+template <typename Add>
+__device__ __forceinline__ void point_stats(float s, double g, Add add) {
   const double lim[7] = {-1e99, 0.0, 0.1, 0.2, 0.5, 1.0, 1e99};
   const float eps_f[3] = {1.f, 1.5f, 2.f};
   const double eps_d[3] = {1.0, 1.5, 2.0};
-  double acc[EV_NSTAT];
+  const double diff = fabs(__dsub_rn((double)s, g));
+  add(0, 1.0);
+  add(1, diff);
 #pragma unroll
-  for (int q = 0; q < EV_NSTAT; ++q) acc[q] = 0.0;
-  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
-    const double g = gt[p];
-    if (!inb[p] || (valid && !valid[p]) || g == 0.0) continue;     // gt_sdf != 0: wall interiors are excluded
-    const float s = pred[p];
-    const double diff = fabs(__dsub_rn((double)s, g));
-    acc[0] += 1.0;
-    acc[1] = __dadd_rn(acc[1], diff);
-#pragma unroll
-    for (int b = 0; b < 6; ++b) {
-      const bool in = g > lim[b] && g < lim[b + 1];
-      acc[2 + b] += in ? 1.0 : 0.0;
-      acc[8 + b] = __dadd_rn(acc[8 + b], in ? diff : 0.0);
-    }
-#pragma unroll
-    for (int e = 0; e < 3; ++e) {
-      const float cp = chomp_f(s, eps_f[e], (float)(eps_d[e] / 2.0), (float)(1.0 / (2.0 * eps_d[e])));
-      acc[14 + e] = __dadd_rn(acc[14 + e], fabs(__dsub_rn((double)cp, chomp_d(g, eps_d[e]))));
-    }
+  for (int b = 0; b < 6; ++b) {
+    const bool in = g > lim[b] && g < lim[b + 1];
+    add(2 + b, in ? 1.0 : 0.0);
+    add(8 + b, in ? diff : 0.0);
   }
-  __shared__ double red[EV_THREADS / 32][EV_NSTAT];
+#pragma unroll
+  for (int e = 0; e < 3; ++e) {
+    const float cp = chomp_f(s, eps_f[e], (float)(eps_d[e] / 2.0), (float)(1.0 / (2.0 * eps_d[e])));
+    add(14 + e, fabs(__dsub_rn((double)cp, chomp_d(g, eps_d[e]))));
+  }
+}
+
+// one block's partials [block][COLS] of the per-thread sums acc: shuffles 16 ... 1 within each warp, then the warps in
+// order
+template <int COLS>
+__device__ __forceinline__ void block_partials(const double (&acc)[COLS], double* __restrict__ partials) {
+  __shared__ double red[EV_THREADS / 32][COLS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-  for (int q = 0; q < EV_NSTAT; ++q) {
+  for (int q = 0; q < COLS; ++q) {
     double v = acc[q];
     for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_down_sync(0xFFFFFFFFu, v, o));
     if (lane == 0) red[warp][q] = v;
   }
   __syncthreads();
-  if (threadIdx.x < EV_NSTAT) {
+  if (threadIdx.x < COLS) {
     double v = 0.0;
     for (int w = 0; w < EV_THREADS / 32; ++w) v = __dadd_rn(v, red[w][threadIdx.x]);
-    partials[(int64_t)blockIdx.x * EV_NSTAT + threadIdx.x] = v;
+    partials[(int64_t)blockIdx.x * COLS + threadIdx.x] = v;
   }
 }
 
-__global__ void stats_final_kernel(const double* __restrict__ partials, int n_blocks, double* __restrict__ out) {
-  if (threadIdx.x >= EV_NSTAT) return;
-  double v = 0.0;
-  for (int b = 0; b < n_blocks; ++b) v = __dadd_rn(v, partials[(int64_t)b * EV_NSTAT + threadIdx.x]);
-  out[threadIdx.x] = v;
-}
-
-// the sums of eval_pts.sub_eval (and of the objects' and the volume's parts of fixed_pts_eval): stats_kernel's 17 sums
-// with nothing left out -- out-of-bounds points carry their fill, GT zeros count -- over [0, n) and, in the same pass,
-// over [0, n_vox); partials [block][2][17], added in block order by stats_final_kernel over 34 columns
-__global__ void __launch_bounds__(EV_THREADS) split_stats_kernel(const float* __restrict__ pred,
-                                                                 const double* __restrict__ gt, int64_t n,
-                                                                 int64_t n_vox, double* __restrict__ partials) {
-  const double lim[7] = {-1e99, 0.0, 0.1, 0.2, 0.5, 1.0, 1e99};
-  const float eps_f[3] = {1.f, 1.5f, 2.f};
-  const double eps_d[3] = {1.0, 1.5, 2.0};
-  double acc[2][EV_NSTAT];
+// ROWS = 1 (eval_sdf): the points in bounds, valid and with gt != 0 (wall interiors are excluded); partials [block][17].
+// ROWS = 2 (eval_pts.sub_eval, and the objects' and the volume's parts of fixed_pts_eval): nothing left out --
+// out-of-bounds points carry their fill, GT zeros count -- row 0 over [0, n), row 1 over [0, n_vox); partials
+// [block][2][17].
+template <int ROWS>
+__global__ void __launch_bounds__(EV_THREADS) stats_kernel(const float* __restrict__ pred, const double* __restrict__ gt,
+                                                           const uint8_t* __restrict__ inb,
+                                                           const uint8_t* __restrict__ valid, int64_t n, int64_t n_vox,
+                                                           double* __restrict__ partials) {
+  double acc[ROWS * EV_NSTAT];
 #pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int q = 0; q < EV_NSTAT; ++q) acc[h][q] = 0.0;
+  for (int q = 0; q < ROWS * EV_NSTAT; ++q) acc[q] = 0.0;
   for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
     const double g = gt[p];
-    const float s = pred[p];
-    const double vox = p < n_vox ? 1.0 : 0.0;
-    double v[EV_NSTAT];
-    const double diff = fabs(__dsub_rn((double)s, g));
-    v[0] = 1.0;
-    v[1] = diff;
-#pragma unroll
-    for (int b = 0; b < 6; ++b) {
-      const bool in = g > lim[b] && g < lim[b + 1];
-      v[2 + b] = in ? 1.0 : 0.0;
-      v[8 + b] = in ? diff : 0.0;
-    }
-#pragma unroll
-    for (int e = 0; e < 3; ++e) {
-      const float cp = chomp_f(s, eps_f[e], (float)(eps_d[e] / 2.0), (float)(1.0 / (2.0 * eps_d[e])));
-      v[14 + e] = fabs(__dsub_rn((double)cp, chomp_d(g, eps_d[e])));
-    }
-#pragma unroll
-    for (int q = 0; q < EV_NSTAT; ++q) {
-      acc[0][q] = __dadd_rn(acc[0][q], v[q]);
-      if (vox != 0.0) acc[1][q] = __dadd_rn(acc[1][q], v[q]);
-    }
+    if (ROWS == 1 && (!inb[p] || (valid && !valid[p]) || g == 0.0)) continue;
+    point_stats(pred[p], g, [&](int q, double v) {
+      acc[q] = __dadd_rn(acc[q], v);
+      if constexpr (ROWS == 2)
+        if (p < n_vox) acc[EV_NSTAT + q] = __dadd_rn(acc[EV_NSTAT + q], v);
+    });
   }
-  __shared__ double red[EV_THREADS / 32][2 * EV_NSTAT];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int q = 0; q < EV_NSTAT; ++q) {
-      double v = acc[h][q];
-      for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_down_sync(0xFFFFFFFFu, v, o));
-      if (lane == 0) red[warp][h * EV_NSTAT + q] = v;
-    }
-  __syncthreads();
-  if (threadIdx.x < 2 * EV_NSTAT) {
-    double v = 0.0;
-    for (int w = 0; w < EV_THREADS / 32; ++w) v = __dadd_rn(v, red[w][threadIdx.x]);
-    partials[(int64_t)blockIdx.x * 2 * EV_NSTAT + threadIdx.x] = v;
-  }
+  block_partials(acc, partials);
 }
 
 // the final sum of a fixed grid's partials [block][cols], column by column in block order
@@ -283,21 +243,12 @@ __global__ void __launch_bounds__(EV_THREADS) cosdist_kernel(const float* __rest
                                                              const double* __restrict__ gt,
                                                              const int64_t* __restrict__ idx, int64_t n, double eps,
                                                              double* __restrict__ partials) {
-  double acc = 0.0;
+  double acc[1] = {0.0};
   for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = idx ? idx[k] : k;
-    acc = __dadd_rn(acc, __dsub_rn(1.0, cos_sim(pred + 3 * k, gt + 3 * r, eps)));
+    acc[0] = __dadd_rn(acc[0], __dsub_rn(1.0, cos_sim(pred + 3 * k, gt + 3 * r, eps)));
   }
-  __shared__ double red[EV_THREADS / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 16; o > 0; o >>= 1) acc = __dadd_rn(acc, __shfl_down_sync(0xFFFFFFFFu, acc, o));
-  if (lane == 0) red[warp] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double v = 0.0;
-    for (int w = 0; w < EV_THREADS / 32; ++w) v = __dadd_rn(v, red[w]);
-    partials[blockIdx.x] = v;
-  }
+  block_partials(acc, partials);
 }
 
 __global__ void visible_kernel(const float* __restrict__ pts, int64_t n, const float* __restrict__ T_CW,
@@ -332,41 +283,78 @@ void eval_destroy(isdfb_ctx* ctx) {
   ctx->eval = nullptr;
 }
 
-int eval_gt_sample(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz, const double* origin,
-                   const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double fill,
-                   double* out, uint8_t* inb, cudaStream_t st) {
+// one thread per point over a lattice with nodes i * spacing + origin: launch(blocks, ax, ay, az, pts) runs the kernel's
+// instantiation for pts_f64 if it is set, else for pts_f32; `entry` names the C-ABI entry in the error message
+template <typename Launch>
+static int lattice_launch(isdfb_ctx* ctx, const char* entry, int nx, int ny, int nz, const double* origin,
+                          const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, Launch launch) {
   if (n == 0) return ISDFB_OK;
-  if ((int64_t)blocks_for(n) > 0x7FFFFFFFLL) ISDFB_FAIL(ctx, ISDFB_ERR_CAPACITY, "isdfb_gt_sdf_sample: %lld points", (long long)n);
+  if ((int64_t)blocks_for(n) > 0x7FFFFFFFLL) ISDFB_FAIL(ctx, ISDFB_ERR_CAPACITY, "%s: %lld points", entry, (long long)n);
   const Axis ax{origin[0], spacing[0], nx}, ay{origin[1], spacing[1], ny}, az{origin[2], spacing[2], nz};
   if (pts_f64)
-    gt_sample_kernel<double><<<blocks_for(n), EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts_f64, n, fill, out, inb);
+    launch(blocks_for(n), ax, ay, az, pts_f64);
   else
-    gt_sample_kernel<float><<<blocks_for(n), EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts_f32, n, fill, out, inb);
+    launch(blocks_for(n), ax, ay, az, pts_f32);
   ISDFB_CUDA_OK(ctx, cudaGetLastError());
   ISDFB_LAUNCHED(ctx);
   return ISDFB_OK;
 }
 
-// ctx->eval: room for the largest partials layout ([block][2][17] of the split statistics)
-static int eval_partials(isdfb_ctx* ctx, double** out) {
-  if (!ctx->eval) ISDFB_CUDA_OK(ctx, cudaMalloc(&ctx->eval, sizeof(double) * EV_STATS_BLOCKS * 2 * EV_NSTAT));
-  *out = (double*)ctx->eval;
-  return ISDFB_OK;
-}
-
 inline int stats_blocks(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(EV_STATS_BLOCKS, blocks_for(n))); }
 
-int eval_error_stats(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, const uint8_t* valid,
-                     int64_t n, double* out, cudaStream_t st) {
-  double* partials;
-  if (int rc = eval_partials(ctx, &partials)) return rc;
+// a reduction on the fixed grid of stats_blocks(n) blocks: launch(blocks, partials) runs the kernel that writes the
+// per-block partials [block][cols], then partials_final_kernel adds them into out[cols].  The partials live in
+// ctx->eval, sized for the largest layout ([block][2][17] of stats_kernel<2>).
+template <typename Launch>
+static int fixed_grid_sum(isdfb_ctx* ctx, int64_t n, int cols, double* out, cudaStream_t st, Launch launch) {
+  if (!ctx->eval) ISDFB_CUDA_OK(ctx, cudaMalloc(&ctx->eval, sizeof(double) * EV_STATS_BLOCKS * 2 * EV_NSTAT));
+  double* partials = (double*)ctx->eval;
   const int nb = stats_blocks(n);
-  stats_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, inb, valid, n, partials);
+  launch(nb, partials);
   ISDFB_CUDA_OK(ctx, cudaGetLastError());
-  stats_final_kernel<<<1, 32, 0, st>>>(partials, nb, out);
+  partials_final_kernel<<<1, (cols + 31) / 32 * 32, 0, st>>>(partials, nb, cols, out);
   ISDFB_CUDA_OK(ctx, cudaGetLastError());
   ctx->launches += 2;
   return ISDFB_OK;
+}
+
+int eval_gt_sample(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz, const double* origin,
+                   const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double fill,
+                   double* out, uint8_t* inb, cudaStream_t st) {
+  return lattice_launch(ctx, "isdfb_gt_sdf_sample", nx, ny, nz, origin, spacing, pts_f32, pts_f64, n,
+                        [&](int nb, Axis ax, Axis ay, Axis az, auto pts) {
+                          gt_sample_kernel<<<nb, EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts, n, fill, out, inb);
+                        });
+}
+
+int eval_gt_grad(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz, const double* origin,
+                 const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double delta,
+                 double* grad, uint8_t* valid, cudaStream_t st) {
+  return lattice_launch(ctx, "isdfb_gt_sdf_grad", nx, ny, nz, origin, spacing, pts_f32, pts_f64, n,
+                        [&](int nb, Axis ax, Axis ay, Axis az, auto pts) {
+                          gt_grad_kernel<<<nb, EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts, n, delta, grad, valid);
+                        });
+}
+
+int eval_error_stats(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, const uint8_t* valid,
+                     int64_t n, double* out, cudaStream_t st) {
+  return fixed_grid_sum(ctx, n, EV_NSTAT, out, st, [&](int nb, double* partials) {
+    stats_kernel<1><<<nb, EV_THREADS, 0, st>>>(pred, gt, inb, valid, n, 0, partials);
+  });
+}
+
+int eval_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, int64_t n, int64_t n_vox, double* out,
+                     cudaStream_t st) {
+  return fixed_grid_sum(ctx, n, 2 * EV_NSTAT, out, st, [&](int nb, double* partials) {
+    stats_kernel<2><<<nb, EV_THREADS, 0, st>>>(pred, gt, nullptr, nullptr, n, n_vox, partials);
+  });
+}
+
+int eval_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* idx, int64_t n, double eps,
+                      double* out, cudaStream_t st) {
+  return fixed_grid_sum(ctx, n, 1, out, st, [&](int nb, double* partials) {
+    cosdist_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, idx, n, eps, partials);
+  });
 }
 
 int eval_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float* T_CW, const float* depth,
@@ -376,46 +364,5 @@ int eval_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float
   visible_kernel<<<blocks_for(n), EV_THREADS, 0, st>>>(pts, n, T_CW, depth, n_frames, H, W, fx, fy, cx, cy, trunc, vis);
   ISDFB_CUDA_OK(ctx, cudaGetLastError());
   ISDFB_LAUNCHED(ctx);
-  return ISDFB_OK;
-}
-
-int eval_gt_grad(isdfb_ctx* ctx, const float* lattice, int nx, int ny, int nz, const double* origin,
-                 const double* spacing, const float* pts_f32, const double* pts_f64, int64_t n, double delta,
-                 double* grad, uint8_t* valid, cudaStream_t st) {
-  if (n == 0) return ISDFB_OK;
-  if ((int64_t)blocks_for(n) > 0x7FFFFFFFLL) ISDFB_FAIL(ctx, ISDFB_ERR_CAPACITY, "isdfb_gt_sdf_grad: %lld points", (long long)n);
-  const Axis ax{origin[0], spacing[0], nx}, ay{origin[1], spacing[1], ny}, az{origin[2], spacing[2], nz};
-  if (pts_f64)
-    gt_grad_kernel<double><<<blocks_for(n), EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts_f64, n, delta, grad, valid);
-  else
-    gt_grad_kernel<float><<<blocks_for(n), EV_THREADS, 0, st>>>(lattice, ax, ay, az, pts_f32, n, delta, grad, valid);
-  ISDFB_CUDA_OK(ctx, cudaGetLastError());
-  ISDFB_LAUNCHED(ctx);
-  return ISDFB_OK;
-}
-
-int eval_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, int64_t n, int64_t n_vox, double* out,
-                     cudaStream_t st) {
-  double* partials;
-  if (int rc = eval_partials(ctx, &partials)) return rc;
-  const int nb = stats_blocks(n);
-  split_stats_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, n, n_vox, partials);
-  ISDFB_CUDA_OK(ctx, cudaGetLastError());
-  partials_final_kernel<<<1, 64, 0, st>>>(partials, nb, 2 * EV_NSTAT, out);
-  ISDFB_CUDA_OK(ctx, cudaGetLastError());
-  ctx->launches += 2;
-  return ISDFB_OK;
-}
-
-int eval_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* idx, int64_t n, double eps,
-                      double* out, cudaStream_t st) {
-  double* partials;
-  if (int rc = eval_partials(ctx, &partials)) return rc;
-  const int nb = stats_blocks(n);
-  cosdist_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, idx, n, eps, partials);
-  ISDFB_CUDA_OK(ctx, cudaGetLastError());
-  partials_final_kernel<<<1, 32, 0, st>>>(partials, nb, 1, out);
-  ISDFB_CUDA_OK(ctx, cudaGetLastError());
-  ctx->launches += 2;
   return ISDFB_OK;
 }

@@ -286,42 +286,54 @@ class Engine:
         return v_out, f_out
 
     # ---- evaluation against a ground-truth SDF -------------------------
+    def _lattice_args(self, lattice, origin, spacing, pts, flat):
+        """Checks the lattice and the points (float32 or float64, [N,3] if flat else [...,3]) of isdfb_gt_sdf_sample and
+        isdfb_gt_sdf_grad.  Returns (lattice, pts, args): the C arguments from the lattice to the point count, and the
+        tensors they point into, which the caller holds until the call (they may be contiguous copies)."""
+        lattice = _f32(lattice, "lattice", self.device)
+        if lattice.dim() != 3:
+            raise ValueError("lattice must be [nx,ny,nz], got %s" % (tuple(lattice.shape),))
+        if (pts.device != self.device or pts.dtype not in (torch.float32, torch.float64) or (flat and pts.dim() != 2)
+                or pts.shape[-1] != 3):
+            raise TypeError("pts must be a float32 or float64 %s tensor on %s" % ("[N,3]" if flat else "[...,3]",
+                                                                                  self.device))
+        pts = pts.contiguous()
+        f64 = pts.dtype == torch.float64
+        args = (_ptr(lattice), *[int(d) for d in lattice.shape], (C.c_double * 3)(*[float(v) for v in origin]),
+                (C.c_double * 3)(*[float(v) for v in spacing]), _ptr(None if f64 else pts), _ptr(pts if f64 else None),
+                pts.numel() // 3)
+        return lattice, pts, args
+
+    def _pred_gt(self, pred, gt):
+        """pred as fp32 [N] and gt as fp64 [N], both contiguous, for the statistics entries."""
+        pred = _f32(pred, "pred", self.device).reshape(-1)
+        if gt.dtype != torch.float64 or gt.device != self.device or gt.numel() != pred.numel():
+            raise TypeError("gt must be float64 on %s with one value per prediction" % self.device)
+        return pred, gt.reshape(-1).contiguous()
+
     def gt_sdf_sample(self, lattice, origin, spacing, pts, fill=0.0):
         """Trilinear interpolation of the fp32 lattice [nx,ny,nz] with nodes i * spacing + origin at pts [...,3]
         (float32 or float64), as scipy's RegularGridInterpolator over sdf_util.get_grid_pts.  Returns (values fp64 [...],
         in-bounds uint8 [...]); out-of-bounds points get `fill`, a NaN coordinate gives NaN and byte 1."""
-        lattice = _f32(lattice, "lattice", self.device)
-        if lattice.dim() != 3:
-            raise ValueError("lattice must be [nx,ny,nz], got %s" % (tuple(lattice.shape),))
-        if pts.device != self.device or pts.dtype not in (torch.float32, torch.float64) or pts.shape[-1] != 3:
-            raise TypeError("pts must be a float32 or float64 [...,3] tensor on %s" % self.device)
-        pts = pts.contiguous()
-        shape = pts.shape[:-1]
-        out = torch.empty(shape, dtype=torch.float64, device=self.device)
-        inb = torch.empty(shape, dtype=torch.uint8, device=self.device)
-        o = (C.c_double * 3)(*[float(v) for v in origin])
-        s = (C.c_double * 3)(*[float(v) for v in spacing])
-        f64 = pts.dtype == torch.float64
-        self._ck(self.lib.isdfb_gt_sdf_sample(self._ctx, _ptr(lattice), *[int(d) for d in lattice.shape], o, s,
-                                              _ptr(None if f64 else pts), _ptr(pts if f64 else None), pts.numel() // 3,
-                                              float(fill), _ptr(out), _ptr(inb), self._stream()))
+        lattice, pts, args = self._lattice_args(lattice, origin, spacing, pts, flat=False)
+        out = torch.empty(pts.shape[:-1], dtype=torch.float64, device=self.device)
+        inb = torch.empty(pts.shape[:-1], dtype=torch.uint8, device=self.device)
+        self._ck(self.lib.isdfb_gt_sdf_sample(self._ctx, *args, float(fill), _ptr(out), _ptr(inb), self._stream()))
         return out, inb
 
     def sdf_error_stats(self, pred, gt, in_bounds, valid=None):
         """The 17 fp64 sums of eval_sdf (device tensor): count, sum |pred - gt|, six bin counts, six bin sums, three
         CHOMP-difference sums, over the points in bounds, valid and with gt != 0."""
-        pred = _f32(pred, "pred", self.device).reshape(-1)
+        pred, gt = self._pred_gt(pred, gt)
         n = pred.numel()
-        if gt.dtype != torch.float64 or gt.device != self.device or gt.numel() != n:
-            raise TypeError("gt must be float64 on %s with one value per prediction" % self.device)
         masks = []
         for t, nm in ((in_bounds, "in_bounds"), (valid, "valid")):
             if t is not None and (t.device != self.device or t.numel() != n):
                 raise ValueError("%s must have one byte per prediction on %s" % (nm, self.device))
             masks.append(None if t is None else t.reshape(-1).to(torch.uint8).contiguous())
         out = torch.empty(17, dtype=torch.float64, device=self.device)
-        self._ck(self.lib.isdfb_sdf_error_stats(self._ctx, _ptr(pred), _ptr(gt.reshape(-1).contiguous()),
-                                                _ptr(masks[0]), _ptr(masks[1]), n, _ptr(out), self._stream()))
+        self._ck(self.lib.isdfb_sdf_error_stats(self._ctx, _ptr(pred), _ptr(gt), _ptr(masks[0]), _ptr(masks[1]), n,
+                                                _ptr(out), self._stream()))
         return out
 
     def points_visible(self, pts, T_CW, depth, fx, fy, cx, cy, trunc):
@@ -343,36 +355,22 @@ class Engine:
         """eval_pts.eval_grad(is_gt_sdf=True) on the lattice of gt_sdf_sample at pts [N,3] (float32 or float64): central
         differences of step delta, NaN where a lookup is outside the lattice or exactly 0.  Returns (grad fp64 [N,3],
         valid uint8 [N], 1 iff no component is NaN)."""
-        lattice = _f32(lattice, "lattice", self.device)
-        if lattice.dim() != 3:
-            raise ValueError("lattice must be [nx,ny,nz], got %s" % (tuple(lattice.shape),))
-        if (pts.device != self.device or pts.dtype not in (torch.float32, torch.float64) or pts.dim() != 2
-                or pts.shape[1] != 3):
-            raise TypeError("pts must be a float32 or float64 [N,3] tensor on %s" % self.device)
-        pts = pts.contiguous()
-        n = pts.shape[0]
-        grad = torch.empty(n, 3, dtype=torch.float64, device=self.device)
-        valid = torch.empty(n, dtype=torch.uint8, device=self.device)
-        o = (C.c_double * 3)(*[float(v) for v in origin])
-        s = (C.c_double * 3)(*[float(v) for v in spacing])
-        f64 = pts.dtype == torch.float64
-        self._ck(self.lib.isdfb_gt_sdf_grad(self._ctx, _ptr(lattice), *[int(d) for d in lattice.shape], o, s,
-                                            _ptr(None if f64 else pts), _ptr(pts if f64 else None), n, float(delta),
-                                            _ptr(grad), _ptr(valid), self._stream()))
+        lattice, pts, args = self._lattice_args(lattice, origin, spacing, pts, flat=True)
+        grad = torch.empty(pts.shape[0], 3, dtype=torch.float64, device=self.device)
+        valid = torch.empty(pts.shape[0], dtype=torch.uint8, device=self.device)
+        self._ck(self.lib.isdfb_gt_sdf_grad(self._ctx, *args, float(delta), _ptr(grad), _ptr(valid), self._stream()))
         return grad, valid
 
     def sdf_split_stats(self, pred, gt, n_vox):
         """eval_pts.sub_eval's sums (device fp64 [2,17]): row 0 over all points, row 1 over the first n_vox, each in
         sdf_error_stats's layout, with no point left out."""
-        pred = _f32(pred, "pred", self.device).reshape(-1)
+        pred, gt = self._pred_gt(pred, gt)
         n = pred.numel()
-        if gt.dtype != torch.float64 or gt.device != self.device or gt.numel() != n:
-            raise TypeError("gt must be float64 on %s with one value per prediction" % self.device)
         if not 0 <= int(n_vox) <= n:
             raise ValueError("n_vox %d outside [0, %d]" % (n_vox, n))
         out = torch.empty(2, 17, dtype=torch.float64, device=self.device)
-        self._ck(self.lib.isdfb_sdf_split_stats(self._ctx, _ptr(pred), _ptr(gt.reshape(-1).contiguous()), n,
-                                                int(n_vox), _ptr(out), self._stream()))
+        self._ck(self.lib.isdfb_sdf_split_stats(self._ctx, _ptr(pred), _ptr(gt), n, int(n_vox), _ptr(out),
+                                                self._stream()))
         return out
 
     def grad_cosdist(self, pred, gt, gt_index=None, eps=1e-6):

@@ -1159,13 +1159,7 @@ class Trainer:
         else:
             (sdf, eval_pts), valid = self.eval_sdf_volume(samples), None
         gt, inb = self.gt_sdf_interp.sample(eval_pts, fill=1e99)
-        st = self.sdf_map.engine().sdf_error_stats(sdf, gt, inb, valid).cpu().numpy()
-        with np.errstate(invalid="ignore", divide="ignore"):
-            av_l1 = st[1] / st[0]
-            binned = st[8:14] / st[2:8]
-            chomp = st[14:17] / st[0]
-        return {"av_l1": float(av_l1), "binned_l1": [float(v) for v in binned],
-                "l1_chomp_costs": [float(v) for v in chomp]}
+        return _stats_result(self.sdf_map.engine().sdf_error_stats(sdf, gt, inb, valid).cpu().numpy())
 
     def _eval_visible(self, samples):
         depth_batch, T_WC_batch = self._eval_frame_data()
@@ -1383,7 +1377,8 @@ class Trainer:
 
 
 def _stats_result(st):
-    """{'av_l1', 'binned_l1', 'l1_chomp_costs'} as floats from the 17 sums of isdfb_sdf_split_stats (0 / 0 = NaN)."""
+    """{'av_l1', 'binned_l1', 'l1_chomp_costs'} as floats from the 17 sums of isdfb_sdf_error_stats or of one row of
+    isdfb_sdf_split_stats (0 / 0 = NaN)."""
     with np.errstate(invalid="ignore", divide="ignore"):
         return {"av_l1": float(st[1] / st[0]), "binned_l1": [float(v) for v in st[8:14] / st[2:8]],
                 "l1_chomp_costs": [float(v) for v in st[14:17] / st[0]]}

@@ -110,6 +110,19 @@ def test_split_stats_match_numpy(eng):
         eng.sdf_split_stats(p, g, n + 1)
 
 
+def test_error_stats_equal_split_stats_row_0(eng):
+    # eval_sdf's and sub_eval's sums share one kernel: where eval_sdf leaves no point out, they agree bitwise
+    rng = np.random.default_rng(14)
+    for n in (1000, 250001):                                         # 4 blocks; the full grid, several points a thread
+        gt = rng.normal(0.3, 0.8, n)
+        gt[:4] = (0.1, 0.2, 0.5, 1.0)                                # on the bin edges: in no bin
+        assert (gt != 0).all()
+        pred = (gt + rng.normal(0, 0.1, n)).astype(np.float32)
+        p, g = torch.from_numpy(pred).to(DEV), torch.from_numpy(gt).to(DEV)
+        inb = torch.ones(n, dtype=torch.uint8, device=DEV)
+        assert torch.equal(eng.sdf_error_stats(p, g, inb), eng.sdf_split_stats(p, g, n // 3)[0])
+
+
 # ---- isdfb_grad_cosdist ---------------------------------------------------------------------------------------------------
 def test_grad_cosdist_matches_torch(eng):
     rng = np.random.default_rng(13)
