@@ -1,32 +1,29 @@
-"""Thin torch <-> C-ABI adapter: owns one `isdfb_ctx`, checks tensors, passes raw device pointers
-and the caller's current CUDA stream.  PyTorch is used for device memory and streams only."""
+"""Thin torch <-> C-ABI adapter: owns one `isdfb_ctx`, checks every tensor it hands to C (`Engine._arg`), passes raw
+device pointers and the caller's current CUDA stream.  PyTorch is used for device memory and streams only."""
 import ctypes as C
 
 import torch
 
 from . import _lib
 
+F32, F64, I32, I64, U8 = torch.float32, torch.float64, torch.int32, torch.int64, torch.uint8
+_SMALL_INTS = (torch.uint8, torch.int8, torch.int16, torch.int32)
+
 
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
-def _f32(t, name, device):
-    if t is None:
-        return None
-    if t.device != device:
-        raise ValueError("%s is on %s, engine is on %s" % (name, t.device, device))
-    if t.dtype != torch.float32:
-        raise TypeError("%s must be float32, got %s" % (name, t.dtype))
-    return t.contiguous()
-
-
-def _i64(t, name, device):
-    if t is None:
-        return None
-    if t.device != device:
-        raise ValueError("%s is on %s, engine is on %s" % (name, t.device, device))
-    return t.to(torch.int64).contiguous()
+def _shape_ok(t, shape, rows):
+    if isinstance(shape, int):
+        ok = t.numel() == shape
+    elif shape is None:
+        ok = True
+    else:
+        want = shape[1:] if shape[0] is ... else shape
+        got = t.shape[max(t.dim() - len(want), 0):] if shape[0] is ... else t.shape
+        ok = len(got) == len(want) and all(w is None or w == g for w, g in zip(want, got))
+    return ok and (rows == 0 or (t.dim() > 0 and t.shape[0] >= rows))
 
 
 class Engine:
@@ -81,25 +78,48 @@ class Engine:
     def _ck(self, rc):
         _lib.check(rc, self._ctx)
 
+    def _arg(self, t, name, dtype, shape=None, rows=0, as_is=False):
+        """`t` as a C entry may receive it, from its metadata alone (no device value is read); None stays None.
+        dtype: one dtype or a tuple of them.  shape: an element count, or a tuple of sizes in which None matches any
+        size and a leading ... any leading axes.  rows: the least size of axis 0, for a buffer reached through an index
+        or a count.  as_is: the entry gets `t` itself, as an output or in-place state must (a copy would lose the
+        write); otherwise `t` is made contiguous, an integer index becomes int64 and a bool mask uint8.  Raises
+        TypeError for the dtype, ValueError for the device, shape or layout."""
+        if t is None:
+            return None
+        if t.device != self.device:
+            raise ValueError("%s is on %s, engine is on %s" % (name, t.device, self.device))
+        dtypes = dtype if isinstance(dtype, tuple) else (dtype,)
+        convert = not as_is and ((dtype == I64 and t.dtype in _SMALL_INTS) or (dtype == U8 and t.dtype == torch.bool))
+        if t.dtype not in dtypes and not convert:
+            raise TypeError("%s must be %s, got %s" % (name, " or ".join(map(str, dtypes)), t.dtype))
+        if not _shape_ok(t, shape, rows):
+            want = "%d elements" % shape if isinstance(shape, int) else "[%s]" % ", ".join(
+                "..." if s is ... else "*" if s is None else str(s) for s in shape)
+            raise ValueError("%s must be %s%s, got %s" % (name, want, " with >= %d rows" % rows if rows else "",
+                                                          list(t.shape)))
+        if as_is and not t.is_contiguous():
+            raise ValueError("%s must be contiguous: the entry writes into it" % name)
+        return t if as_is else t.to(dtypes[0] if convert else t.dtype).contiguous()
+
     @property
     def launches(self):
         return int(self.lib.isdfb_launch_count(self._ctx))
 
     # ---- weights -----------------------------------------------------
     def pack_weights(self, flat):
-        flat = _f32(flat, "params", self.device)
-        if flat.numel() != self.n_params:
-            raise ValueError("expected %d parameters, got %d" % (self.n_params, flat.numel()))
+        flat = self._arg(flat, "params", F32, self.n_params)
         self._ck(self.lib.isdfb_pack_weights(self._ctx, _ptr(flat), self._stream()))
 
     # ---- K1 ----------------------------------------------------------
     def gather_rays(self, depth, normals, ib, ih, iw, cam, frame_map=None, normals_use_frame_map=False):
         dev = self.device
-        depth = _f32(depth, "depth", dev)
-        normals = _f32(normals, "normals", dev)
-        ib, ih, iw = _i64(ib, "indices_b", dev), _i64(ih, "indices_h", dev), _i64(iw, "indices_w", dev)
-        frame_map = _i64(frame_map, "frame_map", dev)
-        n = ib.numel()
+        ib = self._arg(ib, "indices_b", I64, (None,))
+        n = ib.shape[0]
+        ih, iw = self._arg(ih, "indices_h", I64, (n,)), self._arg(iw, "indices_w", I64, (n,))
+        depth = self._arg(depth, "depth", F32, (None, cam.H, cam.W))
+        normals = self._arg(normals, "normals", F32, (None, cam.H, cam.W, 3))
+        frame_map = self._arg(frame_map, "frame_map", I64, (None,))
         d_out = torch.empty(n, dtype=torch.float32, device=dev)
         n_out = torch.empty(n, 3, dtype=torch.float32, device=dev) if normals is not None else None
         valid = torch.empty(n, dtype=torch.uint8, device=dev)
@@ -111,22 +131,18 @@ class Engine:
     def sample_rays(self, T_WC, ib, ih, iw, depth_sample, u_strat, n_near, lin, n_strat, n_surf, cam,
                     min_depth, dist_behind, frame_map=None, dirs_C_in=None, far=None, near=None):
         dev = self.device
-        T_WC = _f32(T_WC, "T_WC", dev)
-        ib, ih, iw = _i64(ib, "indices_b", dev), _i64(ih, "indices_h", dev), _i64(iw, "indices_w", dev)
-        dirs_C_in = _f32(dirs_C_in, "dirs_C", dev)
-        far = _f32(far, "max_depth", dev)
-        near = _f32(near, "min_depth", dev)
-        frame_map = _i64(frame_map, "frame_map", dev)
-        depth_sample = _f32(depth_sample, "depth_sample", dev)
-        u_strat = _f32(u_strat, "u_strat", dev)
-        n_near = _f32(n_near, "n_near", dev)
-        lin = _f32(lin, "lin", dev)
         R = depth_sample.numel() if depth_sample is not None else far.numel()
         S = n_strat + n_surf
-        if u_strat.shape != (R, n_strat):
-            raise ValueError("u_strat must be [%d,%d]" % (R, n_strat))
-        if n_surf > 1 and n_near.shape != (R, n_surf - 1):
-            raise ValueError("n_near must be [%d,%d]" % (R, n_surf - 1))
+        depth_sample, far = self._arg(depth_sample, "depth_sample", F32, R), self._arg(far, "max_depth", F32, R)
+        near = self._arg(near, "min_depth", F32, R)
+        ib, ih = self._arg(ib, "indices_b", I64, R), self._arg(ih, "indices_h", I64, R)
+        iw = self._arg(iw, "indices_w", I64, R)
+        T_WC = self._arg(T_WC, "T_WC", F32, (R if ib is None else None, 4, 4))
+        dirs_C_in = self._arg(dirs_C_in, "dirs_C", F32, (R, 3))
+        frame_map = self._arg(frame_map, "frame_map", I64, (None,))
+        u_strat = self._arg(u_strat, "u_strat", F32, (R, n_strat))
+        n_near = self._arg(n_near, "n_near", F32, (R, max(n_surf - 1, 0)))
+        lin = self._arg(lin, "lin", F32, (None,), rows=n_strat + 1)
         pc = torch.empty(R, S, 3, dtype=torch.float32, device=dev)
         z = torch.empty(R, S, dtype=torch.float32, device=dev)
         dirs_C = torch.empty(R, 3, dtype=torch.float32, device=dev)
@@ -143,10 +159,13 @@ class Engine:
         """K1 fused (fast mode): pixels, gather, depths along rays, world points and the output noise in one
         launch with in-kernel Philox numbers.  Returns the sample dict fields."""
         dev = self.device
-        depth, T_WC = _f32(depth, "depth", dev), _f32(T_WC, "T_WC", dev)
-        normals = _f32(normals, "normals", dev)
-        frame_map = _i64(frame_map, "frame_map", dev)
-        lin = _f32(lin, "lin", dev)
+        frame_map = self._arg(frame_map, "frame_map", I64, (None,), rows=n_frames)
+        F_ = n_frames if frame_map is None else 0          # keyframe rows the slots address without a frame_map
+        depth = self._arg(depth, "depth", F32, (None, cam.H, cam.W), rows=F_)
+        T_WC = self._arg(T_WC, "T_WC", F32, (None, 4, 4), rows=F_)
+        normals = self._arg(normals, "normals", F32, (None, cam.H, cam.W, 3),
+                            rows=F_ if normals_use_frame_map else n_frames)
+        lin = self._arg(lin, "lin", F32, (None,), rows=n_strat + 1)
         R, S = int(n_frames) * int(n_rays), int(n_strat) + int(n_surf)
         i64 = dict(dtype=torch.int64, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
@@ -167,17 +186,15 @@ class Engine:
                     T_WC_sample=T_s, norm_sample=n_s, ray_valid=valid, noise=noise, inv_count_dev=inv)
 
     def ingest_normals(self, depth, cam, out=None):
-        depth = _f32(depth, "depth", self.device)
+        depth = self._arg(depth, "depth", F32, (cam.H, cam.W))
         if out is None:
-            out = torch.empty(*depth.shape, 3, dtype=torch.float32, device=self.device)
-        elif (out.shape != (*depth.shape, 3) or out.dtype != torch.float32 or out.device != self.device
-              or not out.is_contiguous()):
-            raise ValueError("out must be a contiguous float32 [%s, 3] tensor on %s" % (tuple(depth.shape), self.device))
+            out = torch.empty(cam.H, cam.W, 3, dtype=torch.float32, device=self.device)
+        out = self._arg(out, "out", F32, (cam.H, cam.W, 3), as_is=True)
         self._ck(self.lib.isdfb_ingest_normals(self._ctx, _ptr(depth), C.byref(cam), _ptr(out), self._stream()))
         return out
 
     def pe_encode(self, x):
-        x = _f32(x, "x", self.device)
+        x = self._arg(x, "x", F32, (..., 3))
         n = x.numel() // 3
         out = torch.empty(*x.shape[:-1], self.embedding_size, dtype=torch.float32, device=self.device)
         self._ck(self.lib.isdfb_pe_encode(self._ctx, _ptr(x), n, _ptr(out), self._stream()))
@@ -186,14 +203,10 @@ class Engine:
     # ---- K2 / K3 -----------------------------------------------------
     def forward(self, x, noise=None, noise_std=0.0, want_grad=False):
         dev = self.device
-        x = _f32(x, "x", dev)
+        x = self._arg(x, "x", F32, (..., 3))
         shape = x.shape[:-1]
-        if x.shape[-1] != 3:
-            raise ValueError("points must be [...,3]")
         n = x.numel() // 3
-        noise = _f32(noise, "noise", dev)
-        if noise is not None and noise.numel() != n:
-            raise ValueError("noise must have one value per point")
+        noise = self._arg(noise, "noise", F32, n)
         sdf = torch.empty(shape, dtype=torch.float32, device=dev)
         if want_grad:
             g = torch.empty(*shape, 3, dtype=torch.float32, device=dev)
@@ -206,8 +219,8 @@ class Engine:
 
     def forward_grid(self, lin, scale=None, transform=None):
         """K2 over the dim^3 lattice x = T (lin_i s_x, lin_j s_y, lin_k s_z), points generated in-kernel (get_sdf_grid)."""
-        lin = _f32(lin, "lin", self.device)
-        dim = lin.numel()
+        lin = self._arg(lin, "lin", F32, (None,))
+        dim = lin.shape[0]
         sdf = torch.empty(dim, dim, dim, dtype=torch.float32, device=self.device)
         sc = tr = None
         if scale is not None:
@@ -219,28 +232,29 @@ class Engine:
         return sdf
 
     # ---- N4: mesh extraction ------------------------------------------
+    def _cube(self, sdf):
+        d = sdf.shape[0] if sdf.dim() else 0
+        return self._arg(sdf, "sdf", F32, (d, d, d))
+
     def mesh_count(self, sdf):
         """Marching-cubes counts of the lattice sdf [dim,dim,dim] (synchronous): (vertices, faces)."""
-        sdf = _f32(sdf, "sdf", self.device)
-        dim = sdf.shape[0] if sdf.dim() == 3 else -1
-        if sdf.shape != (dim, dim, dim):
-            raise ValueError("sdf must be a [dim,dim,dim] lattice, got %s" % (tuple(sdf.shape),))
+        sdf = self._cube(sdf)
         nv, nf = C.c_int64(), C.c_int64()
-        self._ck(self.lib.isdfb_mesh_count(self._ctx, _ptr(sdf), int(dim), C.byref(nv), C.byref(nf), self._stream()))
+        self._ck(self.lib.isdfb_mesh_count(self._ctx, _ptr(sdf), sdf.shape[0], C.byref(nv), C.byref(nf),
+                                           self._stream()))
         return nv.value, nf.value
 
     def mesh_emit(self, sdf, verts, faces, scale=None, transform=None):
         """Fill verts [V,3] f32 and faces [F,3] int32 with the mesh of the lattice last passed to mesh_count; the
         capacities are the tensors' row counts."""
-        sdf = _f32(sdf, "sdf", self.device)
-        for t, nm, dt in ((verts, "verts", torch.float32), (faces, "faces", torch.int32)):
-            if t.dtype != dt or t.device != self.device or not t.is_contiguous() or t.dim() != 2 or t.shape[1] != 3:
-                raise TypeError("%s must be a contiguous %s [N,3] tensor on %s" % (nm, dt, self.device))
+        sdf = self._cube(sdf)
+        verts = self._arg(verts, "verts", F32, (None, 3), as_is=True)
+        faces = self._arg(faces, "faces", I32, (None, 3), as_is=True)
         sc = (C.c_float * 3)(*[float(v) for v in torch.as_tensor(scale).reshape(-1).tolist()]) if scale is not None else None
         tr = None
         if transform is not None:
             tr = (C.c_float * 12)(*torch.as_tensor(transform, dtype=torch.float32).cpu()[:3, :4].reshape(-1).tolist())
-        self._ck(self.lib.isdfb_mesh_emit(self._ctx, _ptr(sdf), int(sdf.shape[0]), sc, tr, _ptr(verts), verts.shape[0],
+        self._ck(self.lib.isdfb_mesh_emit(self._ctx, _ptr(sdf), sdf.shape[0], sc, tr, _ptr(verts), verts.shape[0],
                                           _ptr(faces), faces.shape[0], self._stream()))
         return verts, faces
 
@@ -254,10 +268,9 @@ class Engine:
     def mesh_cloud(self, depth, T_WC, H_vis, W_vis, fx, fy, cx, cy):
         """Keyframe point cloud of mesh_rec: depth [F,H,W] nearest-resized to (H_vis, W_vis), back-projected with the
         reduced intrinsics, moved to the world.  Returns (cloud [F*H_vis*W_vis, 3], box [6] = min xyz, max xyz)."""
-        depth, T_WC = _f32(depth, "depth", self.device), _f32(T_WC, "T_WC", self.device)
+        depth = self._arg(depth, "depth", F32, (None, None, None))
         F_, H, W = depth.shape
-        if T_WC.shape != (F_, 4, 4):
-            raise ValueError("T_WC must be [%d,4,4]" % F_)
+        T_WC = self._arg(T_WC, "T_WC", F32, (F_, 4, 4))
         cloud = torch.empty(F_ * int(H_vis) * int(W_vis), 3, dtype=torch.float32, device=self.device)
         box = torch.empty(6, dtype=torch.float32, device=self.device)
         self._ck(self.lib.isdfb_mesh_cloud(self._ctx, _ptr(depth), _ptr(T_WC), F_, H, W, int(H_vis), int(W_vis),
@@ -268,13 +281,8 @@ class Engine:
     def mesh_crop(self, cloud, verts, faces, crop_dist):
         """Keep the faces with a vertex closer than crop_dist to the cloud, then the vertices they use (renumbered in
         order).  Returns (vertices [V',3] f32, faces [F',3] int32)."""
-        cloud, verts = _f32(cloud, "cloud", self.device), _f32(verts, "verts", self.device)
-        if faces.dtype != torch.int32 or faces.device != self.device:
-            raise TypeError("faces must be int32 on %s" % self.device)
-        faces = faces.contiguous()
-        for t, nm in ((cloud, "cloud"), (verts, "verts"), (faces, "faces")):
-            if t.dim() != 2 or t.shape[1] != 3:
-                raise ValueError("%s must be [N,3], got %s" % (nm, tuple(t.shape)))
+        cloud = self._arg(cloud, "cloud", F32, (None, 3))
+        verts, faces = self._arg(verts, "verts", F32, (None, 3)), self._arg(faces, "faces", I32, (None, 3))
         nv, nf = verts.shape[0], faces.shape[0]
         kv, kf = C.c_int64(), C.c_int64()
         self._ck(self.lib.isdfb_mesh_crop_count(self._ctx, _ptr(cloud), cloud.shape[0], float(crop_dist), _ptr(verts), nv,
@@ -286,65 +294,44 @@ class Engine:
         return v_out, f_out
 
     # ---- evaluation against a ground-truth SDF -------------------------
-    def _lattice_args(self, lattice, origin, spacing, pts, flat):
-        """Checks the lattice and the points (float32 or float64, [N,3] if flat else [...,3]) of isdfb_gt_sdf_sample and
-        isdfb_gt_sdf_grad.  Returns (lattice, pts, args): the C arguments from the lattice to the point count, and the
-        tensors they point into, which the caller holds until the call (they may be contiguous copies)."""
-        lattice = _f32(lattice, "lattice", self.device)
-        if lattice.dim() != 3:
-            raise ValueError("lattice must be [nx,ny,nz], got %s" % (tuple(lattice.shape),))
-        if (pts.device != self.device or pts.dtype not in (torch.float32, torch.float64) or (flat and pts.dim() != 2)
-                or pts.shape[-1] != 3):
-            raise TypeError("pts must be a float32 or float64 %s tensor on %s" % ("[N,3]" if flat else "[...,3]",
-                                                                                  self.device))
-        pts = pts.contiguous()
-        f64 = pts.dtype == torch.float64
-        args = (_ptr(lattice), *[int(d) for d in lattice.shape], (C.c_double * 3)(*[float(v) for v in origin]),
+    @staticmethod
+    def _lattice_args(lattice, origin, spacing, pts):
+        """The C arguments of isdfb_gt_sdf_sample and isdfb_gt_sdf_grad from the lattice to the point count."""
+        f64 = pts.dtype == F64
+        return (_ptr(lattice), *lattice.shape, (C.c_double * 3)(*[float(v) for v in origin]),
                 (C.c_double * 3)(*[float(v) for v in spacing]), _ptr(None if f64 else pts), _ptr(pts if f64 else None),
                 pts.numel() // 3)
-        return lattice, pts, args
-
-    def _pred_gt(self, pred, gt):
-        """pred as fp32 [N] and gt as fp64 [N], both contiguous, for the statistics entries."""
-        pred = _f32(pred, "pred", self.device).reshape(-1)
-        if gt.dtype != torch.float64 or gt.device != self.device or gt.numel() != pred.numel():
-            raise TypeError("gt must be float64 on %s with one value per prediction" % self.device)
-        return pred, gt.reshape(-1).contiguous()
 
     def gt_sdf_sample(self, lattice, origin, spacing, pts, fill=0.0):
         """Trilinear interpolation of the fp32 lattice [nx,ny,nz] with nodes i * spacing + origin at pts [...,3]
         (float32 or float64), as scipy's RegularGridInterpolator over sdf_util.get_grid_pts.  Returns (values fp64 [...],
         in-bounds uint8 [...]); out-of-bounds points get `fill`, a NaN coordinate gives NaN and byte 1."""
-        lattice, pts, args = self._lattice_args(lattice, origin, spacing, pts, flat=False)
+        lattice = self._arg(lattice, "lattice", F32, (None, None, None))
+        pts = self._arg(pts, "pts", (F32, F64), (..., 3))
         out = torch.empty(pts.shape[:-1], dtype=torch.float64, device=self.device)
         inb = torch.empty(pts.shape[:-1], dtype=torch.uint8, device=self.device)
-        self._ck(self.lib.isdfb_gt_sdf_sample(self._ctx, *args, float(fill), _ptr(out), _ptr(inb), self._stream()))
+        self._ck(self.lib.isdfb_gt_sdf_sample(self._ctx, *self._lattice_args(lattice, origin, spacing, pts),
+                                              float(fill), _ptr(out), _ptr(inb), self._stream()))
         return out, inb
 
     def sdf_error_stats(self, pred, gt, in_bounds, valid=None):
         """The 17 fp64 sums of eval_sdf (device tensor): count, sum |pred - gt|, six bin counts, six bin sums, three
         CHOMP-difference sums, over the points in bounds, valid and with gt != 0."""
-        pred, gt = self._pred_gt(pred, gt)
         n = pred.numel()
-        masks = []
-        for t, nm in ((in_bounds, "in_bounds"), (valid, "valid")):
-            if t is not None and (t.device != self.device or t.numel() != n):
-                raise ValueError("%s must have one byte per prediction on %s" % (nm, self.device))
-            masks.append(None if t is None else t.reshape(-1).to(torch.uint8).contiguous())
+        pred, gt = self._arg(pred, "pred", F32, n), self._arg(gt, "gt", F64, n)
+        in_bounds, valid = self._arg(in_bounds, "in_bounds", U8, n), self._arg(valid, "valid", U8, n)
         out = torch.empty(17, dtype=torch.float64, device=self.device)
-        self._ck(self.lib.isdfb_sdf_error_stats(self._ctx, _ptr(pred), _ptr(gt), _ptr(masks[0]), _ptr(masks[1]), n,
+        self._ck(self.lib.isdfb_sdf_error_stats(self._ctx, _ptr(pred), _ptr(gt), _ptr(in_bounds), _ptr(valid), n,
                                                 _ptr(out), self._stream()))
         return out
 
     def points_visible(self, pts, T_CW, depth, fx, fy, cx, cy, trunc):
         """uint8 [N]: 1 iff some frame of depth [F,H,W] (camera-from-world T_CW [F,4,4]) sees the point within trunc
         behind its surface (frustum.is_visible_torch, any over the frames)."""
-        pts, T_CW, depth = _f32(pts, "pts", self.device), _f32(T_CW, "T_CW", self.device), _f32(depth, "depth", self.device)
-        if pts.dim() != 2 or pts.shape[1] != 3:
-            raise ValueError("pts must be [N,3], got %s" % (tuple(pts.shape),))
+        pts = self._arg(pts, "pts", F32, (None, 3))
+        depth = self._arg(depth, "depth", F32, (None, None, None))
         F_, H, W = depth.shape
-        if T_CW.shape != (F_, 4, 4):
-            raise ValueError("T_CW must be [%d,4,4]" % F_)
+        T_CW = self._arg(T_CW, "T_CW", F32, (F_, 4, 4))
         vis = torch.empty(pts.shape[0], dtype=torch.uint8, device=self.device)
         self._ck(self.lib.isdfb_points_visible(self._ctx, _ptr(pts), pts.shape[0], _ptr(T_CW), _ptr(depth), F_, H, W,
                                                float(fx), float(fy), float(cx), float(cy), float(trunc), _ptr(vis),
@@ -355,17 +342,19 @@ class Engine:
         """eval_pts.eval_grad(is_gt_sdf=True) on the lattice of gt_sdf_sample at pts [N,3] (float32 or float64): central
         differences of step delta, NaN where a lookup is outside the lattice or exactly 0.  Returns (grad fp64 [N,3],
         valid uint8 [N], 1 iff no component is NaN)."""
-        lattice, pts, args = self._lattice_args(lattice, origin, spacing, pts, flat=True)
+        lattice = self._arg(lattice, "lattice", F32, (None, None, None))
+        pts = self._arg(pts, "pts", (F32, F64), (None, 3))
         grad = torch.empty(pts.shape[0], 3, dtype=torch.float64, device=self.device)
         valid = torch.empty(pts.shape[0], dtype=torch.uint8, device=self.device)
-        self._ck(self.lib.isdfb_gt_sdf_grad(self._ctx, *args, float(delta), _ptr(grad), _ptr(valid), self._stream()))
+        self._ck(self.lib.isdfb_gt_sdf_grad(self._ctx, *self._lattice_args(lattice, origin, spacing, pts), float(delta),
+                                            _ptr(grad), _ptr(valid), self._stream()))
         return grad, valid
 
     def sdf_split_stats(self, pred, gt, n_vox):
         """eval_pts.sub_eval's sums (device fp64 [2,17]): row 0 over all points, row 1 over the first n_vox, each in
         sdf_error_stats's layout, with no point left out."""
-        pred, gt = self._pred_gt(pred, gt)
         n = pred.numel()
+        pred, gt = self._arg(pred, "pred", F32, n), self._arg(gt, "gt", F64, n)
         if not 0 <= int(n_vox) <= n:
             raise ValueError("n_vox %d outside [0, %d]" % (n_vox, n))
         out = torch.empty(2, 17, dtype=torch.float64, device=self.device)
@@ -376,19 +365,10 @@ class Engine:
     def grad_cosdist(self, pred, gt, gt_index=None, eps=1e-6):
         """Sum over k of 1 - CosineSimilarity(dim=1, eps)(pred[k], gt[gt_index[k]]) (gt[k] without an index), in fp64
         (device tensor [1]).  pred fp32 [M,3], gt fp64 [N,3], gt_index int64 [M]."""
-        pred = _f32(pred, "pred", self.device)
-        if pred.dim() != 2 or pred.shape[1] != 3:
-            raise ValueError("pred must be [M,3], got %s" % (tuple(pred.shape),))
-        if gt.dtype != torch.float64 or gt.device != self.device or gt.dim() != 2 or gt.shape[1] != 3:
-            raise TypeError("gt must be a float64 [N,3] tensor on %s" % self.device)
-        gt = gt.contiguous()
+        pred = self._arg(pred, "pred", F32, (None, 3))
         m = pred.shape[0]
-        if gt_index is not None:
-            gt_index = _i64(gt_index, "gt_index", self.device).reshape(-1)
-            if gt_index.numel() != m:
-                raise ValueError("gt_index must have one entry per prediction")
-        elif gt.shape[0] != m:
-            raise ValueError("gt must have one row per prediction without gt_index")
+        gt_index = self._arg(gt_index, "gt_index", I64, m)
+        gt = self._arg(gt, "gt", F64, (None if gt_index is not None else m, 3))
         out = torch.empty(1, dtype=torch.float64, device=self.device)
         self._ck(self.lib.isdfb_grad_cosdist(self._ctx, _ptr(pred), _ptr(gt), _ptr(gt_index), m, float(eps), _ptr(out),
                                              self._stream()))
@@ -398,11 +378,10 @@ class Engine:
     def bounds_pc(self, pc, z_vals, depth_sample, ray_valid=None):
         """loss.bounds_pc (loss.py:56-89): bounds [R,S] and target directions [R,S,3] (row 0 unused)."""
         dev = self.device
-        pc, z_vals = _f32(pc, "pc", dev), _f32(z_vals, "z_vals", dev)
-        depth_sample = _f32(depth_sample, "depth_sample", dev)
+        z_vals = self._arg(z_vals, "z_vals", F32, (None, None))
         R, S = z_vals.shape
-        if ray_valid is not None:
-            ray_valid = ray_valid.to(torch.uint8).contiguous()
+        pc, depth_sample = self._arg(pc, "pc", F32, (R, S, 3)), self._arg(depth_sample, "depth_sample", F32, (R,))
+        ray_valid = self._arg(ray_valid, "ray_valid", U8, (R,))
         bounds = torch.empty(R, S, dtype=torch.float32, device=dev)
         vec = torch.empty(R, S, 3, dtype=torch.float32, device=dev)
         self._ck(self.lib.isdfb_bounds_pc(self._ctx, _ptr(pc), _ptr(z_vals), _ptr(depth_sample), _ptr(ray_valid),
@@ -413,21 +392,24 @@ class Engine:
     def train_fwd_bwd(self, pc, z_vals, depth_sample, dirs_C, T_WC_sample, norm_sample, noise, loss_cfg,
                       ray_valid=None, want_grad=True, loss_sums=None):
         dev = self.device
-        pc = _f32(pc, "pc", dev)
+        pc = self._arg(pc, "pc", F32, (None, None, 3))
         R, S = pc.shape[0], pc.shape[1]
-        z_vals = _f32(z_vals, "z_vals", dev)
-        depth_sample = _f32(depth_sample, "depth_sample", dev)
-        dirs_C = _f32(dirs_C, "dirs_C_sample", dev)
-        T_WC_sample = _f32(T_WC_sample, "T_WC_sample", dev)
-        norm_sample = _f32(norm_sample, "norm_sample", dev)
-        noise = _f32(noise, "noise", dev)
-        if ray_valid is not None:
-            ray_valid = ray_valid.to(torch.uint8).contiguous()
+        z_vals = self._arg(z_vals, "z_vals", F32, (R, S))
+        depth_sample = self._arg(depth_sample, "depth_sample", F32, (R,))
+        dirs_C = self._arg(dirs_C, "dirs_C_sample", F32, (R, 3))
+        T_WC_sample = self._arg(T_WC_sample, "T_WC_sample", F32, (R, 4, 4))
+        norm_sample = self._arg(norm_sample, "norm_sample", F32, (R, 3))
+        noise, ray_valid = self._arg(noise, "noise", F32, (R, S)), self._arg(ray_valid, "ray_valid", U8, (R,))
+        # the loss config already holds the raw addresses of its tensors: they are checked, never replaced
+        self._arg(loss_cfg.bounds, "bounds", F32, (R, S), as_is=True)
+        self._arg(loss_cfg.grad_vec, "grad_vec", F32, (R, S, 3), as_is=True)
+        self._arg(loss_cfg.inv_count_tensor, "inv_count_dev", F32, (None,), rows=1, as_is=True)
+        if loss_sums is None:
+            loss_sums = torch.zeros(4, dtype=torch.float32, device=dev)
+        loss_sums = self._arg(loss_sums, "loss_sums", F32, (4,), as_is=True)
         sdf = torch.empty(R, S, dtype=torch.float32, device=dev)
         g = torch.empty(R, S, 3, dtype=torch.float32, device=dev) if want_grad else None
         loss_mat = torch.empty(R, S, dtype=torch.float32, device=dev)
-        if loss_sums is None:
-            loss_sums = torch.zeros(4, dtype=torch.float32, device=dev)
         self._ck(self.lib.isdfb_train_fwd_bwd(self._ctx, _ptr(pc), _ptr(z_vals), _ptr(depth_sample), _ptr(dirs_C),
                                               _ptr(T_WC_sample), _ptr(norm_sample), _ptr(noise), _ptr(ray_valid),
                                               R, S, C.byref(loss_cfg), _ptr(sdf), _ptr(g), _ptr(loss_mat),
@@ -452,6 +434,7 @@ class Engine:
     def export_grads(self, out=None):
         if out is None:
             out = torch.empty(self.n_params, dtype=torch.float32, device=self.device)
+        out = self._arg(out, "out", F32, self.n_params, as_is=True)
         self._ck(self.lib.isdfb_export_grads(self._ctx, _ptr(out), self._stream()))
         return out
 
@@ -464,13 +447,13 @@ class Engine:
     # ---- K5 ----------------------------------------------------------
     def frame_bins(self, loss_mat, ib, ih, iw, n_frames, H, W, factor=8, ray_valid=None):
         dev = self.device
-        loss_mat = _f32(loss_mat, "loss_mat", dev)
-        ib, ih, iw = _i64(ib, "indices_b", dev), _i64(ih, "indices_h", dev), _i64(iw, "indices_w", dev)
+        loss_mat = self._arg(loss_mat, "loss_mat", F32, (None, None))
         R, S = loss_mat.shape
+        ib, ih, iw = (self._arg(ib, "indices_b", I64, (R,)), self._arg(ih, "indices_h", I64, (R,)),
+                      self._arg(iw, "indices_w", I64, (R,)))
+        ray_valid = self._arg(ray_valid, "ray_valid", U8, (R,))
         approx = torch.empty(n_frames, factor, factor, dtype=torch.float32, device=dev)
         favg = torch.empty(n_frames, dtype=torch.float32, device=dev)
-        if ray_valid is not None:
-            ray_valid = ray_valid.to(torch.uint8).contiguous()
         self._ck(self.lib.isdfb_frame_bins(self._ctx, _ptr(loss_mat), _ptr(ray_valid), _ptr(ib), _ptr(ih), _ptr(iw),
                                            R, S, int(n_frames), int(H), int(W), int(factor), _ptr(approx),
                                            _ptr(favg), self._stream()))
@@ -478,17 +461,21 @@ class Engine:
 
     def step_finish(self, loss_mat, ib, ih, iw, n_frames, H, W, factor, ray_valid, frame_map, frame_avg_losses,
                     loss_sums, inv_count, means_out):
-        """K5 + write-back of the per-keyframe losses + the four loss means (clears loss_sums); see the header."""
+        """K5 + write-back of the per-keyframe losses + the four loss means (clears loss_sums); see the header.  It runs
+        inside the captured step, and takes its tensors as they are: only ray_valid may be converted."""
         dev = self.device
+        loss_mat = self._arg(loss_mat, "loss_mat", F32, (None, None), as_is=True)
         R, S = loss_mat.shape
+        ib = self._arg(ib, "indices_b", I64, (R,), as_is=True)
+        ih, iw = self._arg(ih, "indices_h", I64, (R,), as_is=True), self._arg(iw, "indices_w", I64, (R,), as_is=True)
+        ray_valid = self._arg(ray_valid, "ray_valid", U8, (R,))
+        frame_map = self._arg(frame_map, "frame_map", I64, (None,), rows=n_frames, as_is=True)
+        frame_avg_losses = self._arg(frame_avg_losses, "frame_avg_losses", F32, (None,), rows=n_frames, as_is=True)
+        loss_sums = self._arg(loss_sums, "loss_sums", F32, (4,), as_is=True)
+        inv_count = self._arg(inv_count, "inv_count", F32, (None,), rows=1, as_is=True)
+        means_out = self._arg(means_out, "means_out", F32, (4,), as_is=True)
         approx = torch.empty(n_frames, factor, factor, dtype=torch.float32, device=dev)
         favg = torch.empty(n_frames, dtype=torch.float32, device=dev)
-        for t, nm in ((frame_avg_losses, "frame_avg_losses"), (loss_sums, "loss_sums"), (inv_count, "inv_count"),
-                      (means_out, "means_out")):
-            if t is not None and (t.dtype != torch.float32 or t.device != dev or not t.is_contiguous()):
-                raise TypeError("%s must be a contiguous float32 tensor on %s" % (nm, dev))
-        if ray_valid is not None:
-            ray_valid = ray_valid.to(torch.uint8).contiguous()
         self._ck(self.lib.isdfb_step_finish(self._ctx, _ptr(loss_mat), _ptr(ray_valid), _ptr(ib), _ptr(ih), _ptr(iw), R, S,
                                             int(n_frames), int(H), int(W), int(factor), _ptr(approx), _ptr(favg),
                                             _ptr(frame_map), _ptr(frame_avg_losses), _ptr(loss_sums), _ptr(inv_count),
@@ -497,26 +484,28 @@ class Engine:
 
     def select_window(self, frame_avg_losses, n_frames, window_size, seed, out=None):
         """A0 on the device: Gumbel top-k window (see isdfb_select_window)."""
-        w = _f32(frame_avg_losses, "frame_avg_losses", self.device)
+        w = self._arg(frame_avg_losses, "frame_avg_losses", F32, (None,), rows=n_frames)
         if out is None:
             out = torch.empty(window_size, dtype=torch.int64, device=self.device)
+        out = self._arg(out, "out", I64, (window_size,), as_is=True)
         self._ck(self.lib.isdfb_select_window(self._ctx, _ptr(w), int(n_frames), int(window_size),
                                               C.c_uint64(int(seed) & (2 ** 64 - 1)), _ptr(out), self._stream()))
         return out
 
     # ---- K6 ----------------------------------------------------------
+    def _adamw_state(self, params, m, v):
+        n = self.n_params
+        return (_ptr(self._arg(params, "params", F32, n, as_is=True)),
+                _ptr(self._arg(m, "exp_avg", F32, n, as_is=True)), _ptr(self._arg(v, "exp_avg_sq", F32, n, as_is=True)))
+
     def adamw(self, params, m, v, step, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.01, grad_scale=1.0):
-        for t, nm in ((params, "params"), (m, "exp_avg"), (v, "exp_avg_sq")):
-            if t.dtype != torch.float32 or not t.is_contiguous() or t.device != self.device or t.numel() != self.n_params:
-                raise ValueError("%s must be a contiguous float32 [%d] tensor on %s" % (nm, self.n_params, self.device))
-        self._ck(self.lib.isdfb_adamw(self._ctx, _ptr(params), _ptr(m), _ptr(v), int(step), float(lr), float(beta1),
+        self._ck(self.lib.isdfb_adamw(self._ctx, *self._adamw_state(params, m, v), int(step), float(lr), float(beta1),
                                       float(beta2), float(eps), float(weight_decay), float(grad_scale),
                                       self._stream()))
 
-
     def adamw_graph(self, params, m, v, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.01, grad_scale=1.0):
         """K6 with the step counter on the device (CUDA-graph capturable)."""
-        self._ck(self.lib.isdfb_adamw_graph(self._ctx, _ptr(params), _ptr(m), _ptr(v), float(lr), float(beta1),
+        self._ck(self.lib.isdfb_adamw_graph(self._ctx, *self._adamw_state(params, m, v), float(lr), float(beta1),
                                             float(beta2), float(eps), float(weight_decay), float(grad_scale),
                                             self._stream()))
 
@@ -533,6 +522,19 @@ class Engine:
         self._ck(self.lib.isdfb_profile_read(self._ctx, C.byref(c), C.byref(d), C.byref(nc), C.byref(nd)))
         return dict(chain_ms=c.value, dw_ms=d.value, n_chain=nc.value, n_dw=nd.value)
 
+    # ---- debug hook ------------------------------------------------------
+    def debug_buffers(self):
+        """isdfb_debug_buffers: the tensor-core path's raw per-tile side arrays as device addresses (0: absent) with
+        their strides and counts (see the header)."""
+        aux, dhi, dlo, sg = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        a_st, d_st, tiles = C.c_int64(), C.c_int64(), C.c_int64()
+        n_aux, n_dwl = C.c_int32(), C.c_int32()
+        self._ck(self.lib.isdfb_debug_buffers(self._ctx, C.byref(aux), C.byref(a_st), C.byref(dhi), C.byref(dlo),
+                                              C.byref(d_st), C.byref(n_aux), C.byref(n_dwl), C.byref(tiles), C.byref(sg)))
+        return dict(aux=aux.value or 0, aux_stride_floats=a_st.value, dwl_hi=dhi.value or 0, dwl_lo=dlo.value or 0,
+                    dwl_stride_bytes=d_st.value, n_aux=n_aux.value, n_dwl=n_dwl.value, tiles=tiles.value,
+                    sig16=sg.value or 0)
+
 
 class _DevView:
     """Wrap a raw device pointer as a torch tensor through __cuda_array_interface__."""
@@ -544,6 +546,7 @@ class _DevView:
 
 def make_loss_cfg(trunc_weight, trunc_distance, eik_weight, eik_apply_dist, grad_weight, orien_loss, loss_type,
                   noise_std, inv_count, inv_count_dev=None, bounds=None, grad_vec=None):
+    """The loss config of Engine.train_fwd_bwd, which checks the tensors it keeps against the batch."""
     lc = _lib.LossCfg()
     lc.trunc_weight, lc.trunc_distance = float(trunc_weight), float(trunc_distance)
     lc.eik_weight, lc.eik_apply_dist = float(eik_weight), float(eik_apply_dist)
@@ -554,21 +557,12 @@ def make_loss_cfg(trunc_weight, trunc_distance, eik_weight, eik_apply_dist, grad
     lc.loss_type = 1 if loss_type == "L1" else 2
     lc.noise_std = float(noise_std or 0.0)
     lc.inv_count = float(inv_count)
-    lc.inv_count_dev = None
-    if inv_count_dev is not None:
-        if inv_count_dev.dtype != torch.float32 or not inv_count_dev.is_cuda:
-            raise TypeError("inv_count_dev must be a float32 CUDA scalar")
-        lc.inv_count_dev = inv_count_dev.data_ptr()
-        lc._keepalive = inv_count_dev
-    lc.bounds_dev = lc.grad_vec_dev = None
     if (bounds is None) != (grad_vec is None):
         raise ValueError("bounds and grad_vec (the outputs of Engine.bounds_pc) go together")
-    if bounds is not None:
-        for t, nm in ((bounds, "bounds"), (grad_vec, "grad_vec")):
-            if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
-                raise TypeError("%s must be a contiguous float32 CUDA tensor" % nm)
-        lc.bounds_dev, lc.grad_vec_dev = bounds.data_ptr(), grad_vec.data_ptr()
-        lc._keepalive_pc = (bounds, grad_vec)
+    # the struct holds raw addresses: the tensors stay referenced by the config
+    lc.inv_count_tensor, lc.bounds, lc.grad_vec = inv_count_dev, bounds, grad_vec
+    lc.inv_count_dev, lc.bounds_dev, lc.grad_vec_dev = [None if t is None else t.data_ptr()
+                                                        for t in (inv_count_dev, bounds, grad_vec)]
     return lc
 
 
@@ -581,20 +575,16 @@ def make_camera(fx, fy, cx, cy, H, W):
 def debug_state(engine):
     """Test helper: decode the tensor-core path's per-tile side arrays into [points, 256] tensors.
     Returns (aux(arr), dwl(arr) (hi + lo), sig(layer)), each -> fp32 [tiles*128, 256]."""
-    aux, dhi, dlo, sg = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
-    a_st, d_st, tiles = C.c_int64(), C.c_int64(), C.c_int64()
-    n_aux, n_dwl = C.c_int32(), C.c_int32()
-    engine._ck(engine.lib.isdfb_debug_buffers(engine._ctx, C.byref(aux), C.byref(a_st), C.byref(dhi), C.byref(dlo),
-                                              C.byref(d_st), C.byref(n_aux), C.byref(n_dwl), C.byref(tiles), C.byref(sg)))
-    T = tiles.value
-    aux_t = _DevView(aux.value, a_st.value * n_aux.value, engine.device).tensor.view(n_aux.value, T, 64, 128, 4)
+    b = engine.debug_buffers()
+    T, n_aux, n_dwl, d_st = b["tiles"], b["n_aux"], b["n_dwl"], b["dwl_stride_bytes"]
+    aux_t = _DevView(b["aux"], b["aux_stride_floats"] * n_aux, engine.device).tensor.view(n_aux, T, 64, 128, 4)
 
     def raw16(ptr):
-        v = _DevView(ptr, d_st.value * n_dwl.value // 4, engine.device).tensor      # fp32 view of the bytes
-        return v.view(torch.int16).view(n_dwl.value, T, 8, 32, 16, 8)
+        v = _DevView(ptr, d_st * n_dwl // 4, engine.device).tensor      # fp32 view of the bytes
+        return v.view(torch.int16).view(n_dwl, T, 8, 32, 16, 8)
 
-    hi = raw16(dhi.value)
-    lo = raw16(dlo.value) if dlo.value else None
+    hi = raw16(b["dwl_hi"])
+    lo = raw16(b["dwl_lo"]) if b["dwl_lo"] else None
 
     def get_aux(arr, n_tiles):
         return aux_t[arr, :n_tiles].permute(0, 2, 1, 3).reshape(n_tiles * 128, 256).clone()
@@ -608,7 +598,7 @@ def debug_state(engine):
         return h + dec(lo)
 
     def get_sig(layer, n_tiles, n_layers):
-        v = _DevView(sg.value, d_st.value * n_layers // 4, engine.device).tensor.view(torch.int16)
+        v = _DevView(b["sig16"], d_st * n_layers // 4, engine.device).tensor.view(torch.int16)
         v = v.view(n_layers, T, 32, 128, 8)[layer, :n_tiles].permute(0, 2, 1, 3).reshape(n_tiles * 128, 256)
         return (v.to(torch.int32) & 0xFFFF).float() / 65535.0
 

@@ -108,8 +108,8 @@ def sample_along_rays(T_WC, min_depth, max_depth, n_stratified_samples, n_surf_s
     def per_ray(v):
         return v.to(dev).float().reshape(-1).expand(R) if torch.is_tensor(v) else torch.full((R,), float(v), device=dev)
 
-    far = per_ray(max_depth).contiguous()
-    near = per_ray(min_depth).contiguous() if torch.is_tensor(min_depth) else None
+    far = per_ray(max_depth)
+    near = per_ray(min_depth) if torch.is_tensor(min_depth) else None
     if not torch.is_tensor(max_depth) and near is None:
         near = per_ray(min_depth)                     # scalar/scalar: same bins up to the rounding of linspace
     u = torch.rand(R, n_stratified_samples, device=rd).to(dev)
@@ -120,5 +120,5 @@ def sample_along_rays(T_WC, min_depth, max_depth, n_stratified_samples, n_surf_s
     ib = None if T.shape[0] == R else torch.zeros(R, dtype=torch.int64, device=dev)       # one pose for all rays
     pc, z, _, _ = eng.sample_rays(T, ib, None, None, gt_depth if with_surf else None, u, off, lin,
                                   n_stratified_samples, n_surf, cam, 0.0 if near is not None else float(min_depth),
-                                  0.0, dirs_C_in=dirs_C.contiguous(), far=far, near=near)
+                                  0.0, dirs_C_in=dirs_C, far=far, near=near)
     return pc, z

@@ -10,7 +10,6 @@
                                              element (exit status 1) or that all arrays are equal
 The weight gradient and the loss sums are fp32 atomics whose order varies from run to run; they are not dumped."""
 import argparse
-import ctypes as CT
 import os
 import sys
 
@@ -29,18 +28,14 @@ TILE_BYTES = 65536
 
 def side_buffers(eng):
     """The chain kernel's per-tile side buffers as uint8 device tensors, with their array strides and counts."""
-    aux, dhi, dlo, sg = CT.c_void_p(), CT.c_void_p(), CT.c_void_p(), CT.c_void_p()
-    a_st, d_st, tiles = CT.c_int64(), CT.c_int64(), CT.c_int64()
-    n_aux, n_dwl = CT.c_int32(), CT.c_int32()
-    eng._ck(eng.lib.isdfb_debug_buffers(eng._ctx, CT.byref(aux), CT.byref(a_st), CT.byref(dhi), CT.byref(dlo),
-                                        CT.byref(d_st), CT.byref(n_aux), CT.byref(n_dwl), CT.byref(tiles), CT.byref(sg)))
+    b = eng.debug_buffers()
+    a_st, d_st, n_aux, n_dwl = b["aux_stride_floats"] * 4, b["dwl_stride_bytes"], b["n_aux"], b["n_dwl"]
 
     def view(ptr, nbytes):
         return _DevView(ptr, nbytes // 4, eng.device).tensor.view(torch.uint8) if ptr else None
 
-    return dict(aux=view(aux.value, a_st.value * 4 * n_aux.value), aux_stride=a_st.value * 4, n_aux=n_aux.value,
-                dwl_hi=view(dhi.value, d_st.value * n_dwl.value), dwl_lo=view(dlo.value, d_st.value * n_dwl.value),
-                dwl_stride=d_st.value, n_dwl=n_dwl.value, sig16=sg.value)
+    return dict(aux=view(b["aux"], a_st * n_aux), aux_stride=a_st, n_aux=n_aux, dwl_hi=view(b["dwl_hi"], d_st * n_dwl),
+                dwl_lo=view(b["dwl_lo"], d_st * n_dwl), dwl_stride=d_st, n_dwl=n_dwl, sig16=b["sig16"])
 
 
 def dump(eng, mode, cfg, run, n_points, out):
