@@ -233,15 +233,17 @@ int isdfb_step_finish(isdfb_ctx* ctx, const float* loss_mat, const uint8_t* ray_
 /* ---- K6: AdamW + weight re-pack --------------------------------------------------------
  * torch.optim.AdamW.step for the flat parameter vector (trainer.py:435-439, 982) using the
  * ctx-internal gradient times grad_scale (e.g. 1/world_size after the all-reduce), then
- * refreshes the packed weights.  m, v: flat fp32 state; step is 1-based.                    */
-int isdfb_adamw(isdfb_ctx* ctx, float* params_flat, float* m, float* v, int64_t step, float lr,
-                float beta1, float beta2, float eps, float weight_decay, float grad_scale,
+ * refreshes the packed weights.  m, v: flat fp32 state; step is 1-based.  The hyper-parameters
+ * are doubles, as torch's are: 1 - beta2, 1 - lr*wd and the bias corrections are formed in
+ * double and rounded to fp32 once, so p, m and v follow torch's foreach AdamW element by element. */
+int isdfb_adamw(isdfb_ctx* ctx, float* params_flat, float* m, float* v, int64_t step, double lr,
+                double beta1, double beta2, double eps, double weight_decay, float grad_scale,
                 void* stream);
 /* CUDA-graph-safe K6: the 1-based step counter lives on the device (advanced by the call itself), so a
  * captured Trainer.step() replays with the right bias correction.  isdfb_adamw_set_step (synchronous)
  * aligns it with a host-side count (state_dict load, switching from isdfb_adamw).                  */
-int isdfb_adamw_graph(isdfb_ctx* ctx, float* params_flat, float* m, float* v, float lr, float beta1,
-                      float beta2, float eps, float weight_decay, float grad_scale, void* stream);
+int isdfb_adamw_graph(isdfb_ctx* ctx, float* params_flat, float* m, float* v, double lr, double beta1,
+                      double beta2, double eps, double weight_decay, float grad_scale, void* stream);
 int isdfb_adamw_set_step(isdfb_ctx* ctx, int64_t step, void* stream);
 /* ctx-internal gradient buffer (fp32, padded internal layout) for the NCCL all-reduce.     */
 int isdfb_grad_buffer(isdfb_ctx* ctx, float** ptr, int64_t* n_floats);

@@ -36,6 +36,7 @@ P = C.c_void_p
 I64 = C.c_int64
 I32 = C.c_int32
 F = C.c_float
+D = C.c_double
 
 # name -> (restype, argtypes); kept in sync with include/isdf_b200.h (tests/test_abi.py checks it)
 SIGNATURES = {
@@ -66,8 +67,8 @@ SIGNATURES = {
     "isdfb_frame_bins": (C.c_int, [P, P, P, P, P, P, I64, I32, I32, I32, I32, I32, P, P, P]),
     "isdfb_step_finish": (C.c_int, [P, P, P, P, P, P, I64, I32, I32, I32, I32, I32, P, P, P, P, P, P, P, P]),
     "isdfb_select_window": (C.c_int, [P, P, I32, I32, C.c_uint64, P, P]),
-    "isdfb_adamw": (C.c_int, [P, P, P, P, I64, F, F, F, F, F, F, P]),
-    "isdfb_adamw_graph": (C.c_int, [P, P, P, P, F, F, F, F, F, F, P]),
+    "isdfb_adamw": (C.c_int, [P, P, P, P, I64, D, D, D, D, D, F, P]),
+    "isdfb_adamw_graph": (C.c_int, [P, P, P, P, D, D, D, D, D, F, P]),
     "isdfb_adamw_set_step": (C.c_int, [P, I64, P]),
     "isdfb_grad_buffer": (C.c_int, [P, C.POINTER(P), C.POINTER(I64)]),
     "isdfb_mesh_count": (C.c_int, [P, P, I32, C.POINTER(I64), C.POINTER(I64), P]),

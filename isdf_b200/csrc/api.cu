@@ -410,15 +410,15 @@ int isdfb_select_window(isdfb_ctx* ctx, const float* frame_avg_losses, int32_t n
   return sample_select_window(ctx, ctx->sample_dev, frame_avg_losses, n_frames, window_size, seed, frame_map, st);
 }
 
-int isdfb_adamw(isdfb_ctx* ctx, float* params_flat, float* m, float* v, int64_t step, float lr, float beta1,
-                float beta2, float eps, float weight_decay, float grad_scale, void* stream) {
+int isdfb_adamw(isdfb_ctx* ctx, float* params_flat, float* m, float* v, int64_t step, double lr, double beta1,
+                double beta2, double eps, double weight_decay, float grad_scale, void* stream) {
   ENTER(ctx);
   if (!params_flat || !m || !v || step < 1) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_adamw: bad argument");
   return optim_adamw(ctx, params_flat, m, v, step, lr, beta1, beta2, eps, weight_decay, grad_scale, st);
 }
 
-int isdfb_adamw_graph(isdfb_ctx* ctx, float* params_flat, float* m, float* v, float lr, float beta1, float beta2,
-                      float eps, float weight_decay, float grad_scale, void* stream) {
+int isdfb_adamw_graph(isdfb_ctx* ctx, float* params_flat, float* m, float* v, double lr, double beta1, double beta2,
+                      double eps, double weight_decay, float grad_scale, void* stream) {
   ENTER(ctx);
   if (!params_flat || !m || !v) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_adamw_graph: bad argument");
   return optim_adamw_dev(ctx, params_flat, m, v, lr, beta1, beta2, eps, weight_decay, grad_scale, st);

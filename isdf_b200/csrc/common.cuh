@@ -105,10 +105,10 @@ int simt_train(isdfb_ctx* ctx, const float* pc, const float* z_vals, const float
                float* loss_sums, cudaStream_t st);
 int simt_pe_encode(isdfb_ctx* ctx, const float* x, int64_t n, float* out, cudaStream_t st);
 int optim_pack(isdfb_ctx* ctx, const float* params_flat, cudaStream_t st);
-int optim_adamw(isdfb_ctx* ctx, float* params_flat, float* m, float* v, int64_t step, float lr,
-                float b1, float b2, float eps, float wd, float grad_scale, cudaStream_t st);
-int optim_adamw_dev(isdfb_ctx* ctx, float* params_flat, float* m, float* v, float lr, float b1, float b2,
-                    float eps, float wd, float grad_scale, cudaStream_t st);
+int optim_adamw(isdfb_ctx* ctx, float* params_flat, float* m, float* v, int64_t step, double lr,
+                double b1, double b2, double eps, double wd, float grad_scale, cudaStream_t st);
+int optim_adamw_dev(isdfb_ctx* ctx, float* params_flat, float* m, float* v, double lr, double b1, double b2,
+                    double eps, double wd, float grad_scale, cudaStream_t st);
 int optim_set_step(isdfb_ctx* ctx, int64_t step, cudaStream_t st);
 int optim_export_grads(isdfb_ctx* ctx, float* grads_flat, cudaStream_t st);
 int mesh_table_host(uint8_t* rows, int32_t* max_tris);

@@ -122,9 +122,11 @@ __global__ void __launch_bounds__(256) sample_fused_kernel(
     const int64_t f = frame_map ? frame_map[b] : b;
     int h = 0, w = 0;
     if (lane == 0) {
-      const float2 u = make_float2(curand_uniform(&rng), curand_uniform(&rng));      // (0, 1]
-      h = min((int)((1.f - u.x) * (float)cam.H), cam.H - 1);
-      w = min((int)((1.f - u.y) * (float)cam.W), cam.W - 1);
+      // two statements: the order of the draws is the source's (h from word 0, w from word 1), not the compiler's
+      const float uh = curand_uniform(&rng);                                          // (0, 1]
+      const float uw = curand_uniform(&rng);
+      h = min((int)((1.f - uh) * (float)cam.H), cam.H - 1);
+      w = min((int)((1.f - uw) * (float)cam.W), cam.W - 1);
     }
     h = __shfl_sync(0xffffffffu, h, 0);
     w = __shfl_sync(0xffffffffu, w, 0);

@@ -50,6 +50,18 @@ def run_train(engine, sd, batch, noise, cfg, device):
                 pc_bounds=None if pcb is None else pcb.cpu(), pc_vec=None if pcv is None else pcv.cpu())
 
 
+def scatter_flat_grad_into_packed(engine, flat_grads):
+    """Place a gradient given in flat (SDFMap.parameters()) order into the engine's packed gradient buffer by running
+    the library's own export on a probe that numbers the packed positions (the packed layout is internal to the
+    library)."""
+    gb = engine.grad_buffer()
+    assert gb.numel() < 2 ** 24                          # the probe's positions are exact in fp32
+    gb.copy_(torch.arange(1, gb.numel() + 1, device=gb.device, dtype=torch.float32))
+    where = engine.export_grads().round().long() - 1     # flat position -> packed position
+    gb.zero_()
+    gb[where] = flat_grads
+
+
 def rel(a, b):
     a, b = a.double(), b.double()
     return float((a - b).abs().max() / (b.abs().max() + 1e-30))

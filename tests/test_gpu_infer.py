@@ -193,7 +193,7 @@ def test_checkpoint_roundtrip_and_reference_format(seq, tmp_path):
         grads = torch.cat([(torch.randn(p.shape, generator=gg) * 0.01).reshape(-1) for p in tr.sdf_map.parameters()]).to(DEV)
         gb = eng.grad_buffer()
         gb.zero_()
-        _scatter_flat_grad_into_packed(tr, grads)
+        P.scatter_flat_grad_into_packed(eng, grads)
         tr.optimiser.step()
     for k, v in tr.sdf_map.state_dict().items():
         s, sub = gold["model_digest"][k]
@@ -207,21 +207,12 @@ def test_checkpoint_roundtrip_and_reference_format(seq, tmp_path):
     for i, st in gold["opt_digest"].items():
         for key in ("exp_avg", "exp_avg_sq"):
             v = float(mine["optimizer_state_dict"]["state"][i][key].double().sum())
-            assert abs(v - st[key]) < 1e-4 * max(1e-3, abs(st[key])), (i, key)   # fp32 (1-beta2) rounding
+            # K6 follows torch's AdamW element by element; what is left is the fp32 element rounding of torch's CPU
+            # kernels against its CUDA ones, summed in fp64
+            assert abs(v - st[key]) < 1e-6 * max(1e-3, abs(st[key])), (i, key)
         assert float(mine["optimizer_state_dict"]["state"][i]["step"]) == st["step"]
     tr2 = trainer.Trainer("cuda:0", seq, chkpt_load_file=out, precision="fp32")
     tr2.load_optimiser_state(out)
     x = gold["x"].to(DEV)
     assert torch.equal(tr2.sdf_map(x), tr.sdf_map(x)) and tr2.optimiser.step_count == 2
 
-
-def _scatter_flat_grad_into_packed(tr, flat_grads):
-    """Test helper: place a gradient given in SDFMap.parameters() order into the engine's packed gradient buffer by
-    running the library's own export on a one-hot probe (the packed layout is internal to the library)."""
-    eng = tr.sdf_map.engine()
-    gb = eng.grad_buffer()
-    idx = torch.arange(1, gb.numel() + 1, device=DEV, dtype=torch.float32)
-    gb.copy_(idx)                                        # packed position -> value
-    where = eng.export_grads().round().long() - 1        # flat position -> packed position
-    gb.zero_()
-    gb[where] = flat_grads

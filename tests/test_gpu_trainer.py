@@ -85,41 +85,6 @@ def test_state_dict_roundtrip_and_optimizer_state(seq):
     assert torch.allclose(frozen(x), a, atol=1e-6)
 
 
-def test_select_window_matches_the_reference_rule_in_distribution():
-    """A0 on the device (isdfb_select_window) against the reference's rule (trainer.py:652-674): (window-2) older
-    keyframes drawn WITHOUT replacement with p ~ frame_avg_losses via np.random.choice, plus the two latest."""
-    import numpy as np
-    from oracle import isdf_oracle as O
-    from tests import parity as P
-    dev = torch.device("cuda:0")
-    eng = P.make_engine(dev, O.default_cfg(), "fp32", max_points=1024)
-    n, window, draws = 11, 5, 6000
-    w = torch.tensor([0.5, 0.05, 1.5, 0.0, 0.7, 0.25, 1.0, 0.1, 0.9, 123.0, 456.0], device=dev)   # last two are ignored
-    out = torch.empty(draws, window, dtype=torch.int64, device=dev)
-    for s in range(draws):
-        eng.select_window(w, n, window, seed=1000 + s, out=out[s])
-    got = out.cpu().numpy()
-    assert (got[:, -2] == n - 2).all() and (got[:, -1] == n - 1).all()
-    picks = got[:, :window - 2]
-    assert picks.min() >= 0 and picks.max() < n - 2
-    assert all(len(set(r)) == window - 2 for r in picks.tolist())                  # without replacement
-    assert not (picks == 3).any()                                                  # zero-loss keyframe is never drawn
-    p = (w[:n - 2] / w[:n - 2].sum()).cpu().numpy().astype(np.float64)
-    first = np.bincount(picks[:, 0], minlength=n - 2) / draws                      # first pick ~ p exactly
-    assert np.abs(first - p).max() < 4 * np.sqrt(0.25 / draws)
-    rng = np.random.RandomState(5)
-    ref = np.stack([rng.choice(np.arange(n - 2), size=window - 2, replace=False, p=p) for _ in range(20000)])
-    inc_ref = np.bincount(ref.reshape(-1), minlength=n - 2) / 20000.0              # inclusion frequencies
-    inc_got = np.bincount(picks.reshape(-1), minlength=n - 2) / draws
-    assert np.abs(inc_got - inc_ref).max() < 4 * np.sqrt(0.25 / draws) + 4 * np.sqrt(0.25 / 20000)
-    # all-zero history: uniform (the reference would divide 0 / 0)
-    z = torch.zeros(n, device=dev)
-    for s in range(2000):
-        eng.select_window(z, n, window, seed=77 + s, out=out[s])
-    inc0 = np.bincount(out[:2000, :window - 2].cpu().numpy().reshape(-1), minlength=n - 2) / 2000.0
-    assert np.abs(inc0 - (window - 2) / (n - 2)).max() < 4 * np.sqrt(0.25 / 2000)
-
-
 def test_fast_mode_keyframe_decision_ignores_invalid_rays(seq):
     """is_keyframe: rays on zero-depth pixels count neither in the numerator nor in the denominator (the reference
     drops them before the mean, sample.py:49-55); the fixed-shape fast mode must reach the same proportion."""
