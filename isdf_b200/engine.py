@@ -572,34 +572,121 @@ def make_camera(fx, fy, cx, cy, H, W):
     return cam
 
 
-def debug_state(engine):
-    """Test helper: decode the tensor-core path's per-tile side arrays into [points, 256] tensors.
-    Returns (aux(arr), dwl(arr) (hi + lo), sig(layer)), each -> fp32 [tiles*128, 256]."""
-    b = engine.debug_buffers()
-    T, n_aux, n_dwl, d_st = b["tiles"], b["n_aux"], b["n_dwl"], b["dwl_stride_bytes"]
-    aux_t = _DevView(b["aux"], b["aux_stride_floats"] * n_aux, engine.device).tensor.view(n_aux, T, 64, 128, 4)
+def pe_nat_col(c, half):
+    """Internal embedding column -> the reference's column (tc_common.cuh pe_nat_col): [sin_0 cos_0 sin_1 cos_1 ... |
+    x y z | pad] -> [x y z | sin(xb) | sin(xb + pi/2)]; `half` = 21 n_freqs."""
+    if half <= 0:
+        return c
+    if c < 2 * half:
+        return 3 + (c >> 1) + (c & 1) * half
+    if c < 2 * half + 3:
+        return c - 2 * half
+    return c
 
-    def raw16(ptr):
-        v = _DevView(ptr, d_st * n_dwl // 4, engine.device).tensor      # fp32 view of the bytes
-        return v.view(torch.int16).view(n_dwl, T, 8, 32, 16, 8)
 
-    hi = raw16(b["dwl_hi"])
-    lo = raw16(b["dwl_lo"]) if b["dwl_lo"] else None
+class SideState:
+    """Test helper: the tensor-core path's per-tile side state of the LAST chunk it ran, decoded on the device into
+    [points, columns] fp32 tensors.  The array indices are those of tc_create (csrc/tc_path.cu), the element layouts
+    those the chain kernel writes through off_a / off_d / off_x (csrc/tc_chain.cu, tc_common.cuh):
 
-    def get_aux(arr, n_tiles):
-        return aux_t[arr, :n_tiles].permute(0, 2, 1, 3).reshape(n_tiles * 128, 256).clone()
+      aux   fp32 [f/4][128 points][4]:     partial sums 0 .. n_part-1 (3; 6 with two embedding halves), e32 per half,
+                                          h_last, and (strict modes only) zbar2_l for every layer l
+      dW    bf16 [p/16][f/8][16 points][8]: yh_l (0 .. L-1: e, h_0 .. h_{L-2}), ya_l (L ..: abar_e, abar_0 ..),
+                                          xd_l = delta_l, xz_l = zbar_l, v, and with two halves yh_e1, ya_e1;
+                                          hi image always, lo image in bf16x3 only
+      sig16 unorm16 [f/8][128 points][8]: sigma_l for every layer l; in bf16x3g the bf16 zbar2_l image follows at
+                                          layer L + l (same layout)
 
-    def get_dwl(arr, n_tiles, part="sum"):
-        def dec(x):
-            return x[arr, :n_tiles].permute(0, 1, 3, 2, 4).reshape(n_tiles * 128, 256).contiguous().view(torch.bfloat16).float()
-        h = dec(hi)
-        if part == "hi" or lo is None:
-            return h
-        return h + dec(lo)
+    Embedding-fed arrays (e32, yh_0, ya_0 and the second half's) hold the internal column order; `natural` maps them to
+    the reference's.  Rows past the batch's last point are the padded rows of the last tile."""
 
-    def get_sig(layer, n_tiles, n_layers):
-        v = _DevView(b["sig16"], d_st * n_layers // 4, engine.device).tensor.view(torch.int16)
-        v = v.view(n_layers, T, 32, 128, 8)[layer, :n_tiles].permute(0, 2, 1, 3).reshape(n_tiles * 128, 256)
-        return (v.to(torch.int32) & 0xFFFF).float() / 65535.0
+    def __init__(self, engine, n_points):
+        b = engine.debug_buffers()
+        self.L = 2 * engine.block + 2
+        self.E = engine.embedding_size
+        self.NE = 2 if self.E > 256 else 1
+        self.half = 21 * engine.n_freqs
+        self.lean = engine.precision == "bf16x3g"
+        self.n = int(n_points)
+        self.tiles = -(-self.n // 128)
+        self.rows = 128 * self.tiles
+        cap, d_st, L, NE = b["tiles"], b["dwl_stride_bytes"], self.L, self.NE
+        n_part = 6 if NE == 2 else 3
+        # tc_create's indices
+        self.arr_part, self.arr_e32, self.arr_hlast, self.arr_zb2 = 0, n_part, n_part + NE, n_part + NE + 1
+        self.arr_yh, self.arr_ya, self.arr_xd, self.arr_xz, self.arr_v = 0, L, 2 * L, 3 * L, 4 * L
+        self.arr_yh_e1, self.arr_ya_e1 = 4 * L + 1, 4 * L + 2
+        assert b["n_aux"] == n_part + NE + 1 + (0 if self.lean else L), b
+        assert b["n_dwl"] == 4 * L + 1 + (2 if NE == 2 else 0), b
+        assert self.tiles <= cap
+        dev = engine.device
+        self._engine = engine                      # the views below are the context's memory: keep it alive
+        self.has_lo = bool(b["dwl_lo"])
+        self._aux = _DevView(b["aux"], b["aux_stride_floats"] * b["n_aux"], dev).tensor.view(b["n_aux"], cap, 64, 128, 4)
 
-    return get_aux, get_dwl, get_sig
+        def bytes16(ptr, n_arr):
+            return _DevView(ptr, d_st * n_arr // 4, dev).tensor.view(torch.int16)
+
+        self._hi = bytes16(b["dwl_hi"], b["n_dwl"]).view(b["n_dwl"], cap, 8, 32, 16, 8)
+        self._lo = bytes16(b["dwl_lo"], b["n_dwl"]).view(b["n_dwl"], cap, 8, 32, 16, 8) if b["dwl_lo"] else None
+        n_sig = L * (2 if self.lean else 1)
+        self._sig = bytes16(b["sig16"], n_sig).view(n_sig, cap, 32, 128, 8)
+        idx = [pe_nat_col(c, self.half) for c in range(256 * NE)]
+        self._nat_src = torch.tensor([c for c in range(256 * NE) if idx[c] < self.E], device=dev)
+        self._nat_dst = torch.tensor([idx[c] for c in range(256 * NE) if idx[c] < self.E], device=dev)
+
+    # ---- raw arrays, [tiles * 128, 256], internal column order ----
+    def aux(self, arr):
+        return self._aux[arr, :self.tiles].permute(0, 2, 1, 3).reshape(self.rows, 256).clone()
+
+    def dwl(self, arr, part="hi"):
+        """One dW-layout array: part 'hi' or 'lo' (bf16x3 only) as fp32."""
+        src = self._hi if part == "hi" else self._lo
+        if src is None:
+            raise ValueError("no %s image in %s mode" % (part, "bf16x3g" if self.lean else "this"))
+        x = src[arr, :self.tiles].permute(0, 1, 3, 2, 4).reshape(self.rows, 256).contiguous()
+        return x.view(torch.bfloat16).float()
+
+    def sigma_code(self, l):
+        """sigma_l as its unorm16 code (0 .. 65535, int32)."""
+        return self._sig[l, :self.tiles].permute(0, 2, 1, 3).reshape(self.rows, 256).to(torch.int32) & 0xFFFF
+
+    def sigma(self, l):
+        return self.sigma_code(l).float() / 65535.0
+
+    def zbar2(self, l):
+        """zbar2_l: fp32 side array (bf16x3, bf16) or the bf16 image behind sigma (bf16x3g)."""
+        if not self.lean:
+            return self.aux(self.arr_zb2 + l)
+        x = self._sig[self.L + l, :self.tiles].permute(0, 2, 1, 3).reshape(self.rows, 256).contiguous()
+        return x.view(torch.bfloat16).float()
+
+    # ---- embedding-fed arrays ----
+    def natural(self, halves):
+        """Internal columns of the embedding halves (list of [rows, 256]) -> [rows, E] in the reference's order."""
+        x = torch.cat(halves, dim=1)
+        out = torch.zeros(x.shape[0], self.E, dtype=x.dtype, device=x.device)
+        out[:, self._nat_dst] = x[:, self._nat_src]
+        return out
+
+    def e32(self):
+        """The fp32 embedding, [rows, E] natural order."""
+        return self.natural([self.aux(self.arr_e32 + h) for h in range(self.NE)])
+
+    def operand(self, name, l=0, part="hi"):
+        """A weight-gradient operand by name: 'yh' (l = 0: e, l >= 1: h_{l-1}), 'ya' (l = 0: abar_e, l >= 1:
+        abar_{l-1}), 'xd' (delta_l), 'xz' (zbar_l), 'v'.  yh_0 and ya_0 come back as [rows, E] in natural order."""
+        if name == "v":
+            return self.dwl(self.arr_v, part)
+        base = dict(yh=self.arr_yh, ya=self.arr_ya, xd=self.arr_xd, xz=self.arr_xz)[name]
+        if name in ("yh", "ya") and l == 0:
+            halves = [self.dwl(base, part)]
+            if self.NE == 2:
+                halves.append(self.dwl(self.arr_yh_e1 if name == "yh" else self.arr_ya_e1, part))
+            return self.natural(halves)
+        return self.dwl(base + l, part)
+
+
+def debug_state(engine, n_points):
+    """Test helper: the decoded side state of the last chunk (see SideState)."""
+    return SideState(engine, n_points)

@@ -1,6 +1,7 @@
 """Bring-up tool for the tensor-core path (not a pytest): runs K2 / K3 / K4 on a small batch and prints,
 stage by stage, the error of every intermediate (decoded from the per-tile side arrays through
-isdfb_debug_buffers) against the fp64 oracle.  Usage: python tests/tc_debug.py [bf16x3|bf16] [n_rays]"""
+isdfb_debug_buffers, engine.SideState) against the fp64 oracle.  tests/test_gpu_side_state.py holds the same
+comparisons to bounds.  Usage: python tools/tc_debug.py [bf16x3|bf16x3g|bf16] [n_rays] [n_freqs] [block]"""
 import os
 import sys
 
@@ -22,22 +23,25 @@ def rel(a, b):
 
 
 def main():
-    mode = sys.argv[1] if len(sys.argv) > 1 else "bf16x3"
+    mode = sys.argv[1] if len(sys.argv) > 1 else "bf16x3g"
     R = int(sys.argv[2]) if len(sys.argv) > 2 else 10
-    cfg = O.default_cfg(noise_std=0.05, transform=C.rigid_transform(3))
-    sd = C.golden_weights(17, gain=1.5)
+    n_freqs = int(sys.argv[3]) if len(sys.argv) > 3 else 6
+    block = int(sys.argv[4]) if len(sys.argv) > 4 else 2
+    E = 3 + 42 * n_freqs
+    cfg = O.default_cfg(noise_std=0.05, transform=C.rigid_transform(3), n_freqs=n_freqs, block=block)
+    sd = C.golden_weights(17, E=E, block=block, gain=1.5)
     batch, noise = C.loss_batch(18, R)
     n = R * 27
-    nt = (n + 127) // 128
-    L = 6
+    L = 2 * block + 2
+    ic = block + 1
     ref = P.oracle_train(sd, batch, noise, cfg)
-    refi = O.step_sweeps([(w.double(), b.double()) for w, b in O.layers_from_state_dict(sd, 2)],
-                         {k: v.double() for k, v in batch.items()}, dict(cfg, transform=cfg["transform"].double()),
+    layers = [(w.double(), b.double()) for w, b in O.layers_from_state_dict(sd, block)]
+    refi = O.step_sweeps(layers, {k: v.double() for k, v in batch.items()}, dict(cfg, transform=cfg["transform"].double()),
                          noise.double(), keep_intermediates=True)
     eng = P.make_engine(DEV, cfg, mode, max_points=4096)
     eng.pack_weights(P.flat_params(sd, DEV))
     torch.cuda.synchronize()
-    print("== mode", mode, "rays", R, "points", n, "tiles", nt)
+    print("== mode", mode, "rays", R, "points", n, "E", E, "block", block)
 
     x = batch["pc"].reshape(-1, 3).to(DEV)
     nz = noise.reshape(-1).to(DEV)
@@ -52,34 +56,37 @@ def main():
     errs = P.compare_train(out, ref)
     print("K4 train:", {k: ("%.3e" % v if not isinstance(v, list) else ["%.2e" % t for t in v]) for k, v in errs.items()})
 
-    get_aux, get_dwl, get_sig = debug_state(eng)
-    A_ZB2, A_PART, A_E32, A_HL = 0, L, L + 3, L + 4
-    D_YH, D_YA, D_XD, D_XZ, D_V = 0, L, 2 * L, 3 * L, 4 * L
+    st = debug_state(eng, n)
+
+    def op(name, l=0):             # what the weight-gradient kernel reads: hi (+ lo in bf16x3)
+        v = st.operand(name, l)
+        return v + st.operand(name, l, "lo") if st.has_lo else v
 
     def show(name, got, want):
-        want = want[:n]
-        got = got[:n, :want.shape[1]]
-        print("   %-14s rel err %.3e   (ref max %.3e)" % (name, rel(got, want), float(want.abs().max())))
+        print("   %-14s rel err %.3e   (ref max %.3e)" % (name, rel(got[:n], want), float(want.abs().max())))
 
     print("-- intermediates (tile-decoded) vs fp64 oracle")
-    show("e32", get_aux(A_E32, nt), refi["e"])
-    show("Yh[0]=e", get_dwl(D_YH, nt), refi["e"])
+    show("e32", st.e32(), refi["e"])
+    show("Yh[0]=e", op("yh", 0), refi["e"])
     for l in range(L):
-        show("sig[%d]" % l, get_sig(l, nt, L), refi["sig"][l])
+        show("sig[%d]" % l, st.sigma(l), refi["sig"][l])
     for l in range(1, L):
-        show("Yh[%d]=h%d" % (l, l - 1), get_dwl(D_YH + l, nt), refi["inps"][l][:, :256])
-    show("h_last", get_aux(A_HL, nt), refi["h_last"])
+        show("Yh[%d]=h%d" % (l, l - 1), op("yh", l), refi["inps"][l][:, :256])
+    show("h_last", st.aux(st.arr_hlast), refi["h_last"])
+    We = layers[ic][0][:, 256:]
+    show("part cat S1", st.aux(st.arr_part), refi["e"] @ We.t())
     for l in range(L - 1, -1, -1):
-        show("Xd[%d]=delta" % l, get_dwl(D_XD + l, nt), refi["delta"][l])
-    show("Ya[0]=abar_e", get_dwl(D_YA, nt), refi["abar_e"])
+        show("Xd[%d]=delta" % l, op("xd", l), refi["delta"][l])
+    show("Ya[0]=abar_e", op("ya", 0), refi["abar_e"])
+    show("part cat S3", st.aux(st.arr_part + 2), refi["abar_e"] @ We.t())
     for l in range(1, L):
-        show("Ya[%d]=abar%d" % (l, l - 1), get_dwl(D_YA + l, nt), refi["abars"][l - 1])
+        show("Ya[%d]=abar%d" % (l, l - 1), op("ya", l), refi["abars"][l - 1])
     for l in range(L - 1):
-        show("zb2[%d]" % l, get_aux(A_ZB2 + l, nt), refi["zbar2"][l])
+        show("zb2[%d]" % l, st.zbar2(l), refi["zbar2"][l])
     for l in range(L - 1, -1, -1):
-        show("Xz[%d]=zbar" % l, get_dwl(D_XZ + l, nt), refi["zbars"][l])
+        show("Xz[%d]=zbar" % l, op("xz", l), refi["zbars"][l])
     vref = refi["s_bar"].reshape(-1, 1) * refi["h_last"] + refi["abars"][L - 1]
-    show("V", get_dwl(D_V, nt), vref)
+    show("V", op("v"), vref)
 
 
 if __name__ == "__main__":
