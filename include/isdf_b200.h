@@ -364,6 +364,17 @@ int isdfb_sdf_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, i
 int isdfb_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* gt_index, int64_t n,
                        double eps, double* out, void* stream);
 
+/* ---- the collision cost along the future trajectory (Trainer.eval_traj_cost, trainer.py:2010-2052) ----------------
+ * isdfb_chomp_costs: over the points with in_bounds[p] set and gt[p] != 0 (eval_sdf_interp(handle_oob='mask') and the
+ *   zero exclusion; a NaN GT counts), the count and, per epsilon e, the sums of metrics.chomp_cost (metrics.py:95-104)
+ *   of the prediction, computed in fp32 as the reference's torch tensor is, and of the GT in fp64.  pred fp32 [n], gt
+ *   fp64 [n], in_bounds [n] bytes (the mask of isdfb_gt_sdf_sample); eps [n_eps] (host), 1 <= n_eps <=
+ *   ISDFB_CHOMP_MAX_EPS, each > 0 and finite.  out [1 + 2 n_eps] fp64 (device) = [count, pred sums, GT sums], summed in
+ *   fp64 over a grid fixed by n with a fixed-order final sum: two calls agree bitwise.                               */
+#define ISDFB_CHOMP_MAX_EPS 4
+int isdfb_chomp_costs(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* in_bounds, int64_t n,
+                      const double* eps /*[n_eps], host*/, int32_t n_eps, double* out, void* stream);
+
 /* ---- kernel timing (bench.py roofline) ---------------------------------------------------
  * When enabled, the tensor-core path brackets its two kernels (the fused PE+MLP chain kernel and
  * the weight-gradient kernel) with CUDA events on the launching stream.  isdfb_profile_read

@@ -84,6 +84,7 @@ SIGNATURES = {
                                     C.c_double, P, P, P]),
     "isdfb_sdf_split_stats": (C.c_int, [P, P, P, I64, I64, P, P]),
     "isdfb_grad_cosdist": (C.c_int, [P, P, P, P, I64, C.c_double, P, P]),
+    "isdfb_chomp_costs": (C.c_int, [P, P, P, P, I64, C.POINTER(C.c_double), I32, P, P]),
     "isdfb_profile_enable": (C.c_int, [P, I32]),
     "isdfb_profile_read": (C.c_int, [P, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(I64), C.POINTER(I64)]),
     "isdfb_debug_program": (C.c_int, [I32, I32, I32, I32, C.POINTER(I32), I32]),

@@ -523,6 +523,18 @@ int isdfb_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, cons
   return eval_grad_cosdist(ctx, pred, gt, gt_index, n, eps, out, st);
 }
 
+int isdfb_chomp_costs(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* in_bounds, int64_t n,
+                      const double* eps, int32_t n_eps, double* out, void* stream) {
+  ENTER(ctx);
+  if (!out || !eps || n < 0 || (n > 0 && (!pred || !gt || !in_bounds)))
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_chomp_costs: null argument");
+  if (n_eps < 1 || n_eps > ISDFB_CHOMP_MAX_EPS)
+    ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_chomp_costs: %d epsilons, not 1..%d", n_eps, ISDFB_CHOMP_MAX_EPS);
+  for (int e = 0; e < n_eps; ++e)
+    if (!(eps[e] > 0.0) || !isfinite(eps[e])) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_chomp_costs: epsilon %g", eps[e]);
+  return eval_chomp_costs(ctx, pred, gt, in_bounds, n, eps, n_eps, out, st);
+}
+
 int isdfb_debug_mc_table(uint8_t* rows, int32_t* max_tris) {
   NvtxScope _nvtx(__func__);
   if (!rows && !max_tris) return ISDFB_ERR_ARG;

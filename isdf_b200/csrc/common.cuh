@@ -138,3 +138,5 @@ int eval_split_stats(isdfb_ctx* ctx, const float* pred, const double* gt, int64_
                      cudaStream_t st);
 int eval_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const int64_t* idx, int64_t n, double eps,
                       double* out, cudaStream_t st);
+int eval_chomp_costs(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, int64_t n,
+                     const double* eps, int n_eps, double* out, cudaStream_t st);

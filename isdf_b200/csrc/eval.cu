@@ -19,7 +19,9 @@
 //                    which keeps every point and sums [0, n) and [0, n_vox) in one pass.
 // cosdist_kernel     the sum of 1 - torch.nn.CosineSimilarity(dim=1, eps) over pairs of fp32 predicted and fp64 GT
 //                    gradients, the GT row optionally through an index list.
-// partials_final_kernel  the last step of stats_kernel's and cosdist_kernel's reduction: on a grid fixed by n, each
+// chomp_kernel<NE>   Trainer.eval_traj_cost (trainer.py:2010-2052): over the points in bounds with gt != 0, the count
+//                    and per epsilon the sums of chomp_f(pred) and chomp_d(gt), the CHOMP costs of point_stats.
+// partials_final_kernel  the last step of stats_kernel's, cosdist_kernel's and chomp_kernel's reduction: on a grid fixed by n, each
 //                    thread accumulates, block_partials reduces each block by shuffles in a fixed pattern, and this
 //                    kernel adds the per-block partials in block order.  So two calls on the same input agree bitwise.
 // visible_kernel     geometry.frustum.is_visible_torch reduced over the frames (trainer.py:1976-1983): per point and
@@ -210,6 +212,36 @@ __global__ void __launch_bounds__(EV_THREADS) stats_kernel(const float* __restri
   block_partials(acc, partials);
 }
 
+// Trainer.eval_traj_cost: over the points in bounds with gt != 0 (eval_sdf_interp's mask and the zero exclusion), the
+// count and, per epsilon, the sums of metrics.chomp_cost of the fp32 prediction and of the fp64 GT; partials
+// [block][1 + 2 NE] = [count, pred_0 .. pred_NE-1, gt_0 .. gt_NE-1].  A NaN GT counts, as NaN != 0 in the reference.
+template <int NE>
+struct EpsSet {
+  double v[NE];
+};
+
+template <int NE>
+__global__ void __launch_bounds__(EV_THREADS) chomp_kernel(const float* __restrict__ pred, const double* __restrict__ gt,
+                                                           const uint8_t* __restrict__ inb, int64_t n, EpsSet<NE> eps,
+                                                           double* __restrict__ partials) {
+  double acc[1 + 2 * NE];
+#pragma unroll
+  for (int q = 0; q < 1 + 2 * NE; ++q) acc[q] = 0.0;
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
+    const double g = gt[p];
+    if (!inb[p] || g == 0.0) continue;
+    const float s = pred[p];
+    acc[0] = __dadd_rn(acc[0], 1.0);
+#pragma unroll
+    for (int e = 0; e < NE; ++e) {
+      const double ed = eps.v[e];
+      acc[1 + e] = __dadd_rn(acc[1 + e], (double)chomp_f(s, (float)ed, (float)(ed / 2.0), (float)(1.0 / (2.0 * ed))));
+      acc[1 + NE + e] = __dadd_rn(acc[1 + NE + e], chomp_d(g, ed));
+    }
+  }
+  block_partials(acc, partials);
+}
+
 // the final sum of a fixed grid's partials [block][cols], column by column in block order
 __global__ void partials_final_kernel(const double* __restrict__ partials, int n_blocks, int cols,
                                       double* __restrict__ out) {
@@ -355,6 +387,29 @@ int eval_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const
   return fixed_grid_sum(ctx, n, 1, out, st, [&](int nb, double* partials) {
     cosdist_kernel<<<nb, EV_THREADS, 0, st>>>(pred, gt, idx, n, eps, partials);
   });
+}
+
+template <int NE>
+static int chomp_costs_ne(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, int64_t n,
+                          const double* eps, double* out, cudaStream_t st) {
+  static_assert(1 + 2 * NE <= 2 * EV_NSTAT, "the partials buffer holds [block][2 * 17]");
+  EpsSet<NE> es;
+  for (int e = 0; e < NE; ++e) es.v[e] = eps[e];
+  return fixed_grid_sum(ctx, n, 1 + 2 * NE, out, st, [&](int nb, double* partials) {
+    chomp_kernel<NE><<<nb, EV_THREADS, 0, st>>>(pred, gt, inb, n, es, partials);
+  });
+}
+
+int eval_chomp_costs(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, int64_t n,
+                     const double* eps, int n_eps, double* out, cudaStream_t st) {
+  static_assert(ISDFB_CHOMP_MAX_EPS == 4, "one instantiation per epsilon count");
+  switch (n_eps) {
+    case 1: return chomp_costs_ne<1>(ctx, pred, gt, inb, n, eps, out, st);
+    case 2: return chomp_costs_ne<2>(ctx, pred, gt, inb, n, eps, out, st);
+    case 3: return chomp_costs_ne<3>(ctx, pred, gt, inb, n, eps, out, st);
+    case 4: return chomp_costs_ne<4>(ctx, pred, gt, inb, n, eps, out, st);
+  }
+  ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_chomp_costs: %d epsilons", n_eps);
 }
 
 int eval_points_visible(isdfb_ctx* ctx, const float* pts, int64_t n, const float* T_CW, const float* depth,

@@ -374,6 +374,18 @@ class Engine:
                                              self._stream()))
         return out
 
+    def chomp_costs(self, pred, gt, in_bounds, epsilons):
+        """eval_traj_cost's sums (device fp64 [1 + 2 len(epsilons)]): the count of points in bounds with gt != 0, then
+        per epsilon the sum of metrics.chomp_cost over their fp32 predictions, then the same over their fp64 GT."""
+        n = pred.numel()
+        pred, gt = self._arg(pred, "pred", F32, n), self._arg(gt, "gt", F64, n)
+        in_bounds = self._arg(in_bounds, "in_bounds", U8, n)
+        eps = [float(e) for e in epsilons]
+        out = torch.empty(1 + 2 * len(eps), dtype=torch.float64, device=self.device)
+        self._ck(self.lib.isdfb_chomp_costs(self._ctx, _ptr(pred), _ptr(gt), _ptr(in_bounds), n,
+                                            (C.c_double * len(eps))(*eps), len(eps), _ptr(out), self._stream()))
+        return out
+
     # ---- N2 ----------------------------------------------------------
     def bounds_pc(self, pc, z_vals, depth_sample, ray_valid=None):
         """loss.bounds_pc (loss.py:56-89): bounds [R,S] and target directions [R,S,3] (row 0 unused)."""

@@ -17,7 +17,7 @@ Two RNG modes: "reference" consumes torch / numpy generators in exactly the refe
 Visualisation is out of scope (SURVEY.md section 2) and raises; mesh extraction (mesh_rec, write_mesh) runs on the
 device (isdfb_mesh_*), and so does the evaluation against a ground-truth SDF (load_gt_sdf, eval_sdf, eval_object_sdf:
 isdfb_gt_sdf_sample, isdfb_sdf_error_stats, isdfb_points_visible; eval_fixed: isdfb_gt_sdf_grad, isdfb_sdf_split_stats,
-isdfb_grad_cosdist).
+isdfb_grad_cosdist; eval_traj_cost: isdfb_chomp_costs).
 """
 import copy
 import json
@@ -38,7 +38,7 @@ from . import embedding, fc_map, render, sample
 
 _OUT_OF_SCOPE = ("view_sdf", "latest_frame_vis", "update_vis_vars", "frames_vis", "draw_3D", "draw_obj_3D",
                  "obj_slices_vis", "write_slices", "eval_mesh", "compute_slices", "keyframe_vis",
-                 "slices_vis", "render_depth_vis", "render_normals_vis", "to_topdown", "check_gt_sdf", "eval_traj_cost")
+                 "slices_vis", "render_depth_vis", "render_normals_vis", "to_topdown", "check_gt_sdf")
 
 # the evaluation frames' depth transform (eval_pts.get_cache_dataset): fixed scale per format, far values zeroed at 12 m
 _EVAL_DEPTH_SCALE = {"replicaCAD": 1. / 3276.75, "ScanNet": 1. / 1000.}
@@ -47,6 +47,8 @@ _EVAL_FRAME_STRIDE = 5
 _VOX_RES_DIR = {1.: "0.055/", 0.75: "0.063/", 0.5: "0.078/", 0.25: "0.11/"}
 # eval_pts.fixed_pts_eval's literals: samples per point set, near limit, central-difference step, objects' samples
 _FIXED_SAMPLES, _FIXED_MIN_DEPTH, _FIXED_GRAD_DELTA, _FIXED_OBJ_SAMPLES = 200000, 0.1, 0.01, 10000
+# eval_traj_cost's literals: traj.txt rows per second of tot_step_time (not fps) and the CHOMP epsilons
+_TRAJ_POSES_PER_S, _TRAJ_EPSILONS = 30, (1., 1.5, 2.)
 
 
 class GtSdfInterp:
@@ -1235,6 +1237,32 @@ class Trainer:
             keep = inb.bool()
             errors.append(float((gt[keep] - sdf[keep].double()).abs().mean()))
         return errors
+
+    def eval_traj_cost(self, t_ahead=5.):
+        """CHOMP collision cost of the map along the trajectory ahead (trainer.py:2010-2052): the positions of traj.txt's
+        poses [int(30 t), int(min(len - 1, 30 (t + t_ahead)))) with t = tot_step_time (30 poses a second whatever fps
+        is), scored where the GT lattice has a nonzero value.  Returns (pred_costs, gt_costs) for epsilon 1, 1.5, 2:
+        three Python floats summed over the map's fp32 predictions, three np.float64 over the fp64 GT values.  (nan, nan)
+        when the window has fewer than 30 poses or fewer than 90 % of them are scored; None without a traj_file.  The
+        sums are fp64 in a fixed order, so repeated calls agree bitwise."""
+        if not self.traj_file:
+            return None
+        self._need_gt()
+        traj = np.loadtxt(self.traj_file)
+        start = self.tot_step_time * _TRAJ_POSES_PER_S
+        end = min(len(traj) - 1, (self.tot_step_time + t_ahead) * _TRAJ_POSES_PER_S)
+        pts = traj[int(start):int(end)][:, [3, 7, 11]]
+        if len(pts) < _TRAJ_POSES_PER_S:
+            return np.nan, np.nan
+        pts = torch.from_numpy(np.ascontiguousarray(pts)).to(self.device)
+        gt, inb = self.gt_sdf_interp.sample(pts, fill=1e99)          # eval_sdf_interp(handle_oob='mask')
+        with torch.no_grad():
+            sdf = self.sdf_map(pts.float())
+        costs = self.sdf_map.engine().chomp_costs(sdf, gt, inb, _TRAJ_EPSILONS).cpu().numpy()
+        if costs[0] < 0.9 * len(pts):
+            return np.nan, np.nan
+        k = len(_TRAJ_EPSILONS)
+        return [float(c) for c in costs[1:1 + k]], [np.float64(c) for c in costs[1 + k:]]
 
     # ---- the voxblox comparison's fixed-point evaluation (trainer.py:2080-2087, eval/eval_pts.py:96-299) -----------
     def eval_fixed(self):
