@@ -87,10 +87,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-// bring a contiguous global range into L2 ahead of use (no registers, no completion tracking)
-__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- wgmma (warpgroup MMA, accumulators in registers) -------------------------------------------
