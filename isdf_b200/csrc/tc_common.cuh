@@ -87,6 +87,21 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// the same with an L2 cache policy (createpolicy) for the source lines
+__device__ __forceinline__ void bulk_g2s_hint(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+               ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar), "l"(pol)
+               : "memory");
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+// bring a contiguous global range (16-B aligned, a multiple of 16 B) into L2 ahead of use: no registers, no completion
+__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- wgmma (warpgroup MMA, accumulators in registers) -------------------------------------------
