@@ -375,6 +375,46 @@ int isdfb_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, cons
 int isdfb_chomp_costs(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* in_bounds, int64_t n,
                       const double* eps /*[n_eps], host*/, int32_t n_eps, double* out, void* stream);
 
+/* ---- ground-truth SDF lattices from meshes (sdf_util.sdf_from_mesh / sdf_from_mesh_gridgiven / sdf_from_occupancy,
+ * sdf_util.py:312-457) ----------------------------------------------------------------------------------------------
+ * isdfb_voxelize_count: voxelize_subdivide (sdf_util.py:312-368; trimesh.remesh.subdivide_to_size, max_iter 10,
+ *   edge_factor 2).  Every face is split recursively into 4 at its fp64 edge midpoints (a + b) / 2 until none of its
+ *   edges, sqrt(dx^2 + dy^2 + dz^2) in fp64, is longer than max_edge = pitch / 2; every corner of every such leaf
+ *   occupies the voxel rint((v - origin) / pitch) (half to even, as np.round).  SYNCHRONOUS: returns the voxels'
+ *   bounding box, box_lo [3] (host) = the smallest index per axis, box_dims [3] (host) = its size.  verts fp64 [n_verts,3],
+ *   faces [n_faces,3] int32 (faces_int64 = 0) or int64 (1), both on the device.  ISDFB_ERR_ARG: no face, a face index
+ *   outside [0, n_verts), a non-finite vertex of a face, pitch not finite and > 0, a non-finite origin, or a face with
+ *   an edge still over max_edge after ISDFB_VOXELIZE_MAX_DEPTH levels (subdivide_to_size's "max_iter exceeded").
+ *   ISDFB_ERR_CAPACITY: a voxel index over 2^40 in magnitude, a box axis over ISDFB_GT_SDF_MAX_DIM or a box of more than
+ *   2^31 - 1 voxels.
+ * isdfb_voxelize_emit: the same voxels as bytes (1 occupied, 0 empty) into box [box_dims[0], box_dims[1], box_dims[2]]
+ *   (device, C order, caller-allocated, cleared by the call) for the box at box_lo (host); voxels outside the box are
+ *   dropped.  Idempotent stores, no atomics: two calls are bitwise equal.  Call it after a successful count.
+ * isdfb_fill_holes: VoxelGrid.fill = scipy.ndimage.binary_fill_holes with the default structure (6-connectivity), in
+ *   place on box [nx,ny,nz] bytes (device, nonzero = occupied): on return a voxel is 1 iff it was occupied or no path of
+ *   empty face-neighbours joins it to the box border, else 0.  SYNCHRONOUS (the labelling waits for its passes);
+ *   1 <= each axis <= ISDFB_GT_SDF_MAX_DIM, at most 2^31 - 1 voxels.
+ * isdfb_occupancy_sdf: sdf_from_occupancy (sdf_util.py:371-385): sdf = (edt(occ == 0) - edt(occ != 0)) * voxel_size with
+ *   scipy's exact Euclidean distance transform, bit for bit: sqrt_rn of the exact integer squared distance times
+ *   voxel_size, positive at empty voxels, negative at occupied ones.  occ [nx,ny,nz] bytes, sdf [nx,ny,nz] fp64 (device,
+ *   C order).  SYNCHRONOUS (counts the occupied voxels first): an occupancy that is all empty or all occupied is
+ *   ISDFB_ERR_ARG (the transform has no feature to measure to).  1 <= each axis <= ISDFB_GT_SDF_MAX_DIM, so the
+ *   largest squared distance 3 (dim - 1)^2 fits int32; voxel_size finite and > 0.
+ * Workspace, owned by the ctx and grown on demand: 5 bytes per box voxel for the fill, 16 per lattice voxel for the
+ * distance transform.                                                                                               */
+#define ISDFB_VOXELIZE_MAX_DEPTH 9
+#define ISDFB_GT_SDF_MAX_DIM 16384
+int isdfb_voxelize_count(isdfb_ctx* ctx, const double* verts, int64_t n_verts, const void* faces, int32_t faces_int64,
+                         int64_t n_faces, double pitch, const double* origin /*[3], host*/, int64_t* box_lo /*[3], host*/,
+                         int64_t* box_dims /*[3], host*/, void* stream);
+int isdfb_voxelize_emit(isdfb_ctx* ctx, const double* verts, int64_t n_verts, const void* faces, int32_t faces_int64,
+                        int64_t n_faces, double pitch, const double* origin /*[3], host*/,
+                        const int64_t* box_lo /*[3], host*/, const int64_t* box_dims /*[3], host*/, uint8_t* box,
+                        void* stream);
+int isdfb_fill_holes(isdfb_ctx* ctx, uint8_t* box, int32_t nx, int32_t ny, int32_t nz, void* stream);
+int isdfb_occupancy_sdf(isdfb_ctx* ctx, const uint8_t* occ, int32_t nx, int32_t ny, int32_t nz, double voxel_size,
+                        double* sdf, void* stream);
+
 /* ---- kernel timing (bench.py roofline) ---------------------------------------------------
  * When enabled, the tensor-core path brackets its two kernels (the fused PE+MLP chain kernel and
  * the weight-gradient kernel) with CUDA events on the launching stream.  isdfb_profile_read

@@ -85,6 +85,10 @@ SIGNATURES = {
     "isdfb_sdf_split_stats": (C.c_int, [P, P, P, I64, I64, P, P]),
     "isdfb_grad_cosdist": (C.c_int, [P, P, P, P, I64, C.c_double, P, P]),
     "isdfb_chomp_costs": (C.c_int, [P, P, P, P, I64, C.POINTER(C.c_double), I32, P, P]),
+    "isdfb_voxelize_count": (C.c_int, [P, P, I64, P, I32, I64, D, C.POINTER(D), C.POINTER(I64), C.POINTER(I64), P]),
+    "isdfb_voxelize_emit": (C.c_int, [P, P, I64, P, I32, I64, D, C.POINTER(D), C.POINTER(I64), C.POINTER(I64), P, P]),
+    "isdfb_fill_holes": (C.c_int, [P, P, I32, I32, I32, P]),
+    "isdfb_occupancy_sdf": (C.c_int, [P, P, I32, I32, I32, D, P, P]),
     "isdfb_profile_enable": (C.c_int, [P, I32]),
     "isdfb_profile_read": (C.c_int, [P, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(I64), C.POINTER(I64)]),
     "isdfb_debug_program": (C.c_int, [I32, I32, I32, I32, C.POINTER(I32), I32]),
@@ -114,11 +118,18 @@ def load():
     return lib
 
 
+ERR_ARG, ERR_CUDA, ERR_CAPACITY, ERR_STATE = -1, -2, -3, -4
+
+
 class IsdfbError(RuntimeError):
-    pass
+    """A C entry's failure; `rc` is its isdfb_status."""
+
+    def __init__(self, msg, rc=None):
+        super().__init__(msg)
+        self.rc = rc
 
 
 def check(rc, ctx=None):
     if rc != 0:
         msg = load().isdfb_last_error(ctx)
-        raise IsdfbError("isdf_b200 error %d: %s" % (rc, msg.decode() if msg else "?"))
+        raise IsdfbError("isdf_b200 error %d: %s" % (rc, msg.decode() if msg else "?"), rc)

@@ -160,6 +160,7 @@ int isdfb_destroy(isdfb_ctx* ctx) {
   if (ctx->sample_dev) cudaFree(ctx->sample_dev);
   mesh_destroy(ctx);
   eval_destroy(ctx);
+  gt_sdf_destroy(ctx);
   delete ctx;
   return ISDFB_OK;
 }
@@ -533,6 +534,32 @@ int isdfb_chomp_costs(isdfb_ctx* ctx, const float* pred, const double* gt, const
   for (int e = 0; e < n_eps; ++e)
     if (!(eps[e] > 0.0) || !isfinite(eps[e])) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_chomp_costs: epsilon %g", eps[e]);
   return eval_chomp_costs(ctx, pred, gt, in_bounds, n, eps, n_eps, out, st);
+}
+
+int isdfb_voxelize_count(isdfb_ctx* ctx, const double* verts, int64_t n_verts, const void* faces, int32_t faces_int64,
+                         int64_t n_faces, double pitch, const double* origin, int64_t* box_lo, int64_t* box_dims,
+                         void* stream) {
+  ENTER(ctx);
+  if (!box_lo || !box_dims) ISDFB_FAIL(ctx, ISDFB_ERR_ARG, "isdfb_voxelize_count: null argument");
+  return gt_voxelize_count(ctx, verts, n_verts, faces, faces_int64, n_faces, pitch, origin, box_lo, box_dims, st);
+}
+
+int isdfb_voxelize_emit(isdfb_ctx* ctx, const double* verts, int64_t n_verts, const void* faces, int32_t faces_int64,
+                        int64_t n_faces, double pitch, const double* origin, const int64_t* box_lo,
+                        const int64_t* box_dims, uint8_t* box, void* stream) {
+  ENTER(ctx);
+  return gt_voxelize_emit(ctx, verts, n_verts, faces, faces_int64, n_faces, pitch, origin, box_lo, box_dims, box, st);
+}
+
+int isdfb_fill_holes(isdfb_ctx* ctx, uint8_t* box, int32_t nx, int32_t ny, int32_t nz, void* stream) {
+  ENTER(ctx);
+  return gt_fill_holes(ctx, box, nx, ny, nz, st);
+}
+
+int isdfb_occupancy_sdf(isdfb_ctx* ctx, const uint8_t* occ, int32_t nx, int32_t ny, int32_t nz, double voxel_size,
+                        double* sdf, void* stream) {
+  ENTER(ctx);
+  return gt_occupancy_sdf(ctx, occ, nx, ny, nz, voxel_size, sdf, st);
 }
 
 int isdfb_debug_mc_table(uint8_t* rows, int32_t* max_tris) {

@@ -70,6 +70,7 @@ struct isdfb_ctx {
   void* sample_dev;        // device FusedSampleState {step, valid, blocks_done} of the fused fast-mode sampler
   void* mesh;              // mesh extraction workspace (mesh.cu), created by the first isdfb_mesh_* call, grows on demand
   void* eval;              // per-block partial sums of the eval.cu reductions, allocated on first use
+  void* gtsdf;             // voxelizer / fill / EDT workspace (gt_sdf.cu), created by the first call, grows on demand
 };
 
 extern char g_isdfb_create_err[512];
@@ -140,3 +141,13 @@ int eval_grad_cosdist(isdfb_ctx* ctx, const float* pred, const double* gt, const
                       double* out, cudaStream_t st);
 int eval_chomp_costs(isdfb_ctx* ctx, const float* pred, const double* gt, const uint8_t* inb, int64_t n,
                      const double* eps, int n_eps, double* out, cudaStream_t st);
+void gt_sdf_destroy(isdfb_ctx* ctx);
+int gt_voxelize_count(isdfb_ctx* ctx, const double* verts, int64_t n_verts, const void* faces, int faces_int64,
+                      int64_t n_faces, double pitch, const double* origin, int64_t* box_lo, int64_t* box_dims,
+                      cudaStream_t st);
+int gt_voxelize_emit(isdfb_ctx* ctx, const double* verts, int64_t n_verts, const void* faces, int faces_int64,
+                     int64_t n_faces, double pitch, const double* origin, const int64_t* box_lo,
+                     const int64_t* box_dims, uint8_t* box, cudaStream_t st);
+int gt_fill_holes(isdfb_ctx* ctx, uint8_t* box, int nx, int ny, int nz, cudaStream_t st);
+int gt_occupancy_sdf(isdfb_ctx* ctx, const uint8_t* occ, int nx, int ny, int nz, double voxel_size, double* sdf,
+                     cudaStream_t st);

@@ -1,1 +1,1 @@
-from . import data_util, dataset  # noqa: F401
+from . import data_util, dataset, sdf_util  # noqa: F401

@@ -386,6 +386,41 @@ class Engine:
                                             (C.c_double * len(eps))(*eps), len(eps), _ptr(out), self._stream()))
         return out
 
+    # ---- ground-truth SDF lattices from meshes ---------------------------
+    def _mesh_args(self, verts, faces, pitch, origin):
+        """The C arguments of isdfb_voxelize_count / _emit from the vertices to the origin."""
+        verts = self._arg(verts, "verts", F64, (None, 3))
+        faces = self._arg(faces, "faces", (I64, I32), (None, 3))
+        org = (C.c_double * 3)(*[float(v) for v in origin])
+        return (_ptr(verts), verts.shape[0], _ptr(faces), int(faces.dtype == I64), faces.shape[0], float(pitch), org), \
+            (verts, faces)
+
+    def voxelize(self, verts, faces, pitch, origin=(0., 0., 0.)):
+        """voxelize_subdivide (sdf_util.py:312-368): the voxels rint((v - origin) / pitch) of every corner of the faces
+        subdivided until no edge exceeds pitch / 2.  verts fp64 [V,3], faces int32 or int64 [F,3].  Returns (box_lo, a
+        tuple of 3 ints: the smallest voxel index per axis; box uint8 [dx,dy,dz], 1 at the occupied voxels)."""
+        args, keep = self._mesh_args(verts, faces, pitch, origin)
+        lo, dims = (C.c_int64 * 3)(), (C.c_int64 * 3)()
+        self._ck(self.lib.isdfb_voxelize_count(self._ctx, *args, lo, dims, self._stream()))
+        box = torch.empty(tuple(dims), dtype=torch.uint8, device=self.device)
+        self._ck(self.lib.isdfb_voxelize_emit(self._ctx, *args, lo, dims, _ptr(box), self._stream()))
+        return tuple(lo), box
+
+    def fill_holes(self, box):
+        """scipy.ndimage.binary_fill_holes (6-connectivity) in place on the uint8 box [nx,ny,nz]; returns it (0 / 1)."""
+        box = self._arg(box, "box", U8, (None, None, None), as_is=True)
+        self._ck(self.lib.isdfb_fill_holes(self._ctx, _ptr(box), *box.shape, self._stream()))
+        return box
+
+    def occupancy_sdf(self, occ, voxel_size):
+        """sdf_from_occupancy (sdf_util.py:371-385): (edt(occ == 0) - edt(occ != 0)) * voxel_size in fp64 [nx,ny,nz],
+        bitwise scipy's; occ uint8 or bool [nx,ny,nz], neither all empty nor all occupied."""
+        occ = self._arg(occ, "occ", U8, (None, None, None))
+        sdf = torch.empty(occ.shape, dtype=torch.float64, device=self.device)
+        self._ck(self.lib.isdfb_occupancy_sdf(self._ctx, _ptr(occ), *occ.shape, float(voxel_size), _ptr(sdf),
+                                              self._stream()))
+        return sdf
+
     # ---- N2 ----------------------------------------------------------
     def bounds_pc(self, pc, z_vals, depth_sample, ray_valid=None):
         """loss.bounds_pc (loss.py:56-89): bounds [R,S] and target directions [R,S,3] (row 0 unused)."""
