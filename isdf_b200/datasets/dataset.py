@@ -2,7 +2,8 @@
 
 `SyntheticStream` is the seeded synthetic stream of SURVEY.md 8d (the real sequences are not
 available offline); `ReplicaDataset` reads the reference's ReplicaCAD on-disk layout
-(reference isdf/datasets/dataset.py:20-71: results/depth%06d.png, frame%06d.png, traj.txt)."""
+(reference isdf/datasets/dataset.py:20-71: results/depth%06d.png, frame%06d.png, traj.txt), `ScanNetDataset` its ScanNet
+layout and `RealsenseFrankaOffline` its recorded Franka tabletop sequences."""
 import math
 import os
 
@@ -113,6 +114,45 @@ class ScanNetDataset:
         if depth is None or image is None:
             raise FileNotFoundError("missing ScanNet frame %d under %s" % (idx, self.root_dir))
         T = self.Ts[idx] if self.Ts is not None else None
+        if self.rgb_transform:
+            image = self.rgb_transform(image)
+        if self.depth_transform:
+            depth = self.depth_transform(depth)
+        return {"image": image, "depth": depth, "T": T}
+
+
+class RealsenseFrankaOffline:
+    """Recorded Franka tabletop sequences of the reference (datasets/dataset.py:123-173): <root>/depth/%05d.npy (uint16
+    millimetres as the recorder writes them), <root>/rgb/%05d<col_ext>, and `traj_file` rows of a timestamp followed by
+    the 16 entries of the pose.  Unlike the reference the constructor does not change the process's working directory:
+    a relative `root_dir` or `traj_file` is resolved against the current directory, as for the other readers."""
+
+    def __init__(self, root_dir, traj_file, rgb_transform=None, depth_transform=None, col_ext=".jpg",
+                 noisy_depth=None, distortion_coeffs=None, camera_matrix=None):
+        if traj_file is None:
+            raise ValueError("RealsenseFrankaOffline needs traj_file: the recorded poses (timestamp + 16 values per row) "
+                             "are the only source of the camera poses")
+        self.root_dir = root_dir
+        self.rgb_dir = os.path.join(root_dir, "rgb")
+        self.depth_dir = os.path.join(root_dir, "depth")
+        self.Ts = np.loadtxt(traj_file, ndmin=2)[:, 1:].reshape(-1, 4, 4)
+        self.rgb_transform, self.depth_transform, self.col_ext = rgb_transform, depth_transform, col_ext or ".jpg"
+
+    def __len__(self):
+        return self.Ts.shape[0]
+
+    def __getitem__(self, idx):
+        import cv2
+        idx = int(idx)
+        s = "%05d" % idx
+        depth_file = os.path.join(self.depth_dir, s + ".npy")
+        if not os.path.isfile(depth_file):
+            raise FileNotFoundError("missing Franka depth frame %s" % depth_file)
+        depth = np.load(depth_file)
+        image = cv2.imread(os.path.join(self.rgb_dir, s + self.col_ext))
+        if image is None:
+            raise FileNotFoundError("missing Franka frame %s under %s" % (s + self.col_ext, self.rgb_dir))
+        T = self.Ts[idx]
         if self.rgb_transform:
             image = self.rgb_transform(image)
         if self.depth_transform:

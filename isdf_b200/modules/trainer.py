@@ -225,6 +225,8 @@ class Trainer:
         if self.dataset_format == "realsense_franka_offline":
             self.set_scene_properties()                # trainer.py:82-83: workspace box from the config
         self.load_networks()
+        if self.incremental is False:
+            self.add_data(self.get_data(self.indices))     # the views load_data chose (trainer.py:510-528)
         if chkpt_load_file is not None:
             self.load_checkpoint(chkpt_load_file)
         self.sdf_map.train()
@@ -418,9 +420,19 @@ class Trainer:
             self.scene_dataset = ds.ScanNetDataset(self.scannet_dir, traj_file=self.traj_file, rgb_transform=ds.bgr_to_rgb,
                                                    depth_transform=depth_tf, col_ext=".jpg")
             self._depth_is_metric = True
+        elif fmt == "realsense_franka_offline":
+            self.up = np.array([0., 0., 1.])
+            camera_matrix = np.array([[self.fx, 0.0, self.cx], [0.0, self.fy, self.cy], [0.0, 0.0, 1.0]])
+            # the reader does not undistort (neither does the reference's); the calibration is handed on unused
+            self.scene_dataset = ds.RealsenseFrankaOffline(self.ims_file, traj_file=self.traj_file,
+                                                           rgb_transform=ds.bgr_to_rgb, depth_transform=depth_tf,
+                                                           col_ext=".jpg", distortion_coeffs=self.distortion_coeffs,
+                                                           camera_matrix=camera_matrix)
+            self._depth_is_metric = True
         else:
-            raise NotImplementedError("dataset format %r: only 'synthetic', 'replicaCAD', 'replica' and 'ScanNet' readers "
-                                      "are provided (live / ROS ingest is outside the hot path)" % fmt)
+            raise NotImplementedError("dataset format %r: only the 'synthetic', 'replicaCAD', 'replica', 'ScanNet' and "
+                                      "'realsense_franka_offline' readers are provided; 'arkit', 'realsense' and "
+                                      "'realsense_franka' (live ingest) are not" % fmt)
         if self.incremental is False:
             if self.indices is None:
                 n_views = self.config["dataset"].get("n_views", 0)
@@ -428,8 +440,9 @@ class Trainer:
                 self.indices = (np.random.choice(np.arange(0, n), size=n_views, replace=False)
                                 if self.config["dataset"].get("random_views") else
                                 np.linspace(0, n, n_views, dtype=int, endpoint=False))
+            # the constructor reads these views once the map exists (fast-mode ingest estimates the normals with the
+            # map's engine); the reference reads them here
             self.last_is_keyframe = True
-            self.add_data(self.get_data(self.indices))
 
     def get_data(self, idxs):
         """Host frames -> device FrameData (+ per-pixel normals when the normal loss is on).
